@@ -1,8 +1,8 @@
 #!/usr/bin/env python
-"""bench.py -- simulated events per wall-second of the hot path on B200 (BASELINE.json metric).
+"""bench.py -- simulated events per wall-second of the hot path on one H100 (BASELINE.json metric).
 
 Workload at N=1 (--config 1, the default): BASELINE.json configs[1], "65 536 independent M/M/1
-replicas, 1e6 sim seconds, 1xB200" (Source.poisson(8) -> Server(Exponential(0.1)) -> Sink).  One STEP
+replicas, 1e6 sim seconds" on one GPU (Source.poisson(8) -> Server(Exponential(0.1)) -> Sink).  One STEP
 advances every replica by one window of simulated time (default 1e4 s of the 1e6 s horizon, about
 3.96e10 events at 65 536 replicas): consecutive steps are consecutive windows of ONE continuing run
 (state resident in HBM, resumed by the kernel), exactly the reference's Simulation._run_window slicing;
@@ -30,7 +30,7 @@ CPU oracle and compares their summaries, entity statistics and -- in record mode
 byte for byte: the number printed is for a run whose results are the reference's.
 
 --impl reference times the reference's own CPU path on the host cores: the UNMODIFIED Python reference
-(installed by the recipe in DESIGN.md section 8 into baseline/_ref, which travels to the GPU box) through its
+(installed into oracle/_ref by build() from the reference checkout, oracle/Makefile target `ref`) through its
 own ParallelRunner(max_workers=cores).run_replicas, kind "reference"; if that install is missing, the C
 restatement (oracle port) on all cores, kind "port".  The port's figure is reported next to it either way.
 """
@@ -53,7 +53,7 @@ METRIC = "simulated_events_per_second"
 UNIT = "events/s"
 RATE, MEAN = 8.0, 0.1
 BYTES_EVENT, BYTES_SAMPLE, BYTES_SERVICE = 16, 16, 8
-REF_DIR = os.path.join(ROOT, "baseline", "_ref")
+REF_DIR = os.path.join(ROOT, "oracle", "_ref")
 
 
 def parse():
@@ -73,7 +73,50 @@ def parse():
     ap.add_argument("--no-other-mode", action="store_true")
     ap.add_argument("--no-other-configs", action="store_true")
     ap.add_argument("--no-e2e-records", action="store_true")
+    ap.add_argument("--dump-outputs", metavar="DIR", default=None,
+                    help="write what the timed run returned after its last step as DIR/<name>.npy (float64, < 64 MB)")
     return ap.parse_args()
+
+
+DUMP_KEY_BYTES = 10 << 20          # per output; six outputs at most, so a dump stays under 64 MB
+DUMP_SEED = 20240917
+
+
+def dump_outputs(out, n, directory):
+    """The per-replica outputs a caller of Engine.read_outputs() receives, one float64 .npy per field:
+    DIR/<output>.<field>.npy, replicas along the first axis.  An output whose fields of all n replicas take at most
+    DUMP_KEY_BYTES is written whole; a larger one for the first k replicas (k as many as fit) of a permutation drawn
+    with a fixed seed, in ascending order, their indices in DIR/<output>.replicas.npy.  Every 64-bit integer field is
+    written as its exact 32-bit halves <field>_hi / <field>_lo (of the two's-complement bit pattern), whatever its
+    values, so the file names depend only on the outputs present.  Returns the bytes written."""
+    import numpy as np
+    os.makedirs(directory, exist_ok=True)
+    order = np.random.default_rng(DUMP_SEED).permutation(n)
+    arrays = {}
+    for key in ("summaries", "entity_stats", "records", "sink_samples", "service_samples", "histograms"):
+        a = out.get(key)
+        if a is None:
+            continue
+        cols = []
+        for f in a.dtype.names or (None,):
+            if f == "pad":
+                continue
+            v = a if f is None else a[f]
+            name = key if f is None else f"{key}.{f}"
+            if v.dtype.kind in "iu" and v.dtype.itemsize == 8:
+                u = v.view(np.uint64)
+                cols += [(name + "_hi", u >> np.uint64(32)), (name + "_lo", u & np.uint64(0xFFFFFFFF))]
+            else:
+                cols.append((name, v))
+        per_replica = sum(c[0].size for _, c in cols) * 8
+        if per_replica * n > DUMP_KEY_BYTES:
+            idx = np.sort(order[:max(1, DUMP_KEY_BYTES // per_replica)])
+            arrays[f"{key}.replicas"] = idx
+            cols = [(name, c[idx]) for name, c in cols]
+        arrays.update(cols)
+    for name, v in arrays.items():
+        np.save(os.path.join(directory, f"{name}.npy"), np.ascontiguousarray(v, dtype=np.float64))
+    return sum(v.size * 8 for v in arrays.values())
 
 
 def peaks():
@@ -81,7 +124,7 @@ def peaks():
         with open(os.path.join(ROOT, "MEASURED_PEAKS.json")) as f:
             return float(json.load(f)["hbm_gbs"]), "measured (MEASURED_PEAKS.json)"
     except Exception:
-        return 6650.0, "fallback (B200_PROFILING.md)"
+        return 3350.0, "fallback (H100 SXM data sheet, 3.35 TB/s HBM3; not measured)"
 
 
 def host_cores():
@@ -106,7 +149,7 @@ def host_cores():
 
 
 class ClockSampler:
-    """nvidia-smi clocks/throttle reasons during the timed region (B200_PROFILING.md recipe)."""
+    """nvidia-smi clocks/throttle reasons during the timed region (read-only queries)."""
     Q = ("index,clocks.sm,clocks.max.sm,power.draw,clocks_event_reasons.active,"
          "clocks_event_reasons.hw_slowdown,clocks_event_reasons.hw_thermal_slowdown,"
          "clocks_event_reasons.sw_thermal_slowdown,clocks_event_reasons.sw_power_cap")
@@ -179,7 +222,7 @@ def workload_config(a, cfg, world):
             "replicas_per_gpu": cfg["replicas"], "replicas_total": cfg["replicas"] * world, "window_s": cfg["window_s"],
             "horizon_s": cfg["horizon_s"], "step": "one window of simulated time for every replica (resumed state)",
             "mode": cfg["mode"], "parallelism": f"replicas sharded over {world} GPU(s), no data-path collective",
-            "l2": "working set (replica state + queue rings + recorder rings) > 126 MB L2; no explicit flush"
+            "l2": "working set (replica state + queue rings + recorder rings) > 50 MB L2; no explicit flush"
                   if a.config == 1 else "working set (per-replica state blocks) read and written once per window"}
 
 
@@ -245,7 +288,7 @@ def cpu_reference_throughput(budget_s, cores, seed):
     v = ev / dt
     return {"value": v, "unit": UNIT, "cores": cores, "kind": "reference", "per_core": v / cores,
             "sample": f"{n} M/M/1 replicas x {sim_s:g} sim-s ({ev:.3e} events, {dt:.1f} s wall incl. pool start-up) on the "
-                      f"unmodified Python reference (baseline/_ref), ParallelRunner(max_workers={cores}).run_replicas"}, ev, dt
+                      f"unmodified Python reference (oracle/_ref), ParallelRunner(max_workers={cores}).run_replicas"}, ev, dt
 
 
 def run_reference_arm(a, rank, world):
@@ -282,9 +325,10 @@ def run_reference_arm(a, rank, world):
             "vs_baseline": None, "dtype": "f64", "data": "synthetic", "config": workload_config(a, cfg, 1),
             "cpu_baseline": cb, "cpu_baseline_port": port,
             "e2e": {"value": value, "unit": UNIT, "h2d_bytes_per_step": 0, "d2h_bytes_per_step": 0},
-            "note": ("the unmodified Python reference (baseline/_ref) through its own ParallelRunner on all usable host "
+            "note": ("the unmodified Python reference (oracle/_ref) through its own ParallelRunner on all usable host "
                      "cores, each step a bounded sample of configs[1]'s workload" if use_ref else
-                     "baseline/_ref is not installed on this box: the reference arm is its C restatement (oracle port, "
+                     "the reference is not installed in oracle/_ref (build() without the reference checkout): the reference arm "
+                     "is its C restatement (oracle port, "
                      "pinned event-by-event against the reference) on all usable host cores") +
                     "; cpu_baseline_port is the C port on the same cores for comparison"}
     print(json.dumps(line), flush=True)
@@ -382,6 +426,8 @@ def main():
         clk.start()
     res = timed_run(cfg["mode"], a.steps, a.warmup)
     clocks = clk.stop() if rank == 0 else None
+    if a.dump_outputs and rank == 0:
+        dump_outputs(eng.read_outputs(), n, a.dump_outputs)
 
     def reduce_max(x):
         if world == 1:

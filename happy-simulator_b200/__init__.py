@@ -1,8 +1,8 @@
-"""happysim_b200 -- B200-native engine behind the happy-simulator modelling API.
+"""happysim_b200 -- H100-native engine behind the happy-simulator modelling API.
 
 The hot path of the reference (``Simulation.run()``'s pop-invoke-push loop over
 a heapq of Python ``Event`` objects, happysimulator/core/simulation.py:449-505)
-runs here as hand-written sm_100a CUDA behind a C-ABI (include/hs_b200.h);
+runs here as hand-written sm_90a CUDA behind a C-ABI (include/hs_b200.h);
 this package is the thin Python host side: the modelling classes users already
 write against, the lowering of their object graph to a flat model table, and
 the ctypes binding.  There is NO CPU fallback: without the CUDA library and a

@@ -1,4 +1,4 @@
-"""Build the CUDA engine in-tree: happy-simulator_b200/libhs_b200.so (sm_100a)."""
+"""Build the CUDA engine in-tree: happy-simulator_b200/libhs_b200.so (sm_90a, H100)."""
 from __future__ import annotations
 
 import os
@@ -10,7 +10,7 @@ CSRC = os.path.join(PKG_DIR, "csrc")
 LIB_PATH = os.environ.get("HS_B200_LIB") or os.path.join(PKG_DIR, "libhs_b200.so")
 
 NVCC_FLAGS = [
-    "-gencode", "arch=compute_100a,code=sm_100a", "-O3", "-lineinfo", "-std=c++17",
+    "-gencode", "arch=compute_90a,code=sm_90a", "-O3", "-lineinfo", "-std=c++17",
     "-Xcompiler", "-fPIC", "-shared",
 ]
 

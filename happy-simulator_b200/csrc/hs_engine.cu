@@ -1,4 +1,4 @@
-/* hs_engine.cu -- C-ABI of the B200 discrete-event engine (include/hs_b200.h).
+/* hs_engine.cu -- C-ABI of the H100 discrete-event engine (include/hs_b200.h).
  *
  * Host side of the boundary: validates and uploads the flat model, owns the
  * device buffers (replica state, queue rings, per-replica outputs), picks the
@@ -65,7 +65,7 @@ struct hs_engine {
     bool own_stream = false;
     cudaEvent_t ev0 = nullptr, ev1 = nullptr;
     uint64_t launches = 0;
-    int sm_count = 148;
+    int sm_count = 132;
 
     /* model (host copy + device copy) */
     bool have_model = false;

@@ -144,25 +144,36 @@ struct hs_lane_out {
     uint32_t *hist;                   /* [replica][HS_HIST_BINS] or NULL */
 };
 
-/* 256-bit global store (sm_100a: STG.E.256), one full 32-byte sector per lane.  The recorder streams
- * are write-once per ring pass, so they bypass L1 and are marked evict-first in L2 (HS_ST256_POLICY
- * 0 selects the default write-back policy; kept as a compile-time switch for A/B measurements). */
+/* 256-bit global store: one full 32-byte sector per lane, written as two back-to-back 128-bit stores
+ * (STG.E.128, the widest global store of sm_90a) to the two halves of the sector.  The recorder streams
+ * are write-once per ring pass, so they are written with the streaming policy (st.global.cs,
+ * HS_ST256_POLICY 2).  1 selects L1 no-allocate + an L2 evict-first cache policy, 0 the default
+ * write-back policy; kept as a compile-time switch for A/B measurements.  tools/bench_lane.py on one
+ * H100 80GB HBM3 (400 W power limit), record mode, 65 536 replicas: 2 -> 37.1e9, 1 -> 35.3e9,
+ * 0 -> 32.2e9 events/s (profiles/h100_lane_store_policy_ab.txt). */
 #ifndef HS_ST256_POLICY
-#define HS_ST256_POLICY 1
+#define HS_ST256_POLICY 2
 #endif
 #ifndef HS_LANE_PREDICATED
 #define HS_LANE_PREDICATED 1    /* SIMPLE chains: state updates as selects + predicated memory operations (0: two branches) */
 #endif
-__device__ __forceinline__ void hs_st256(void *p, const uint4 a, const uint4 b)
+__device__ __forceinline__ void hs_st128(void *p, const uint4 a)
 {
 #if HS_ST256_POLICY == 1
-    asm volatile("st.global.L1::no_allocate.L2::evict_first.v8.b32 [%0], {%1,%2,%3,%4,%5,%6,%7,%8};"
+    asm volatile("{\n\t.reg .b64 pol;\n\t"
+                 "createpolicy.fractional.L2::evict_first.b64 pol, 1.0;\n\t"
+                 "st.global.L1::no_allocate.L2::cache_hint.v4.b32 [%0], {%1,%2,%3,%4}, pol;\n\t}"
 #elif HS_ST256_POLICY == 2
-    asm volatile("st.global.cs.v8.b32 [%0], {%1,%2,%3,%4,%5,%6,%7,%8};"
+    asm volatile("st.global.cs.v4.b32 [%0], {%1,%2,%3,%4};"
 #else
-    asm volatile("st.global.v8.b32 [%0], {%1,%2,%3,%4,%5,%6,%7,%8};"
+    asm volatile("st.global.v4.b32 [%0], {%1,%2,%3,%4};"
 #endif
-                 :: "l"(p), "r"(a.x), "r"(a.y), "r"(a.z), "r"(a.w), "r"(b.x), "r"(b.y), "r"(b.z), "r"(b.w) : "memory");
+                 :: "l"(p), "r"(a.x), "r"(a.y), "r"(a.z), "r"(a.w) : "memory");
+}
+__device__ __forceinline__ void hs_st256(void *p, const uint4 a, const uint4 b)
+{
+    hs_st128(p, a);
+    hs_st128((uint4 *)p + 1, b);
 }
 
 /* next arrival of a constant-rate profile, with the reference's "time travel" outcome
@@ -596,11 +607,11 @@ hs_lane_kernel(hs_lane_model M, hs_lane_run P, hs_lane_state *__restrict__ state
                     }
                     if ((FLAGS & HS_LF_REC) && rec) st_wr += nrec;
                 }
-                /* Two forms of the same updates, chosen per kernel by measurement (tools/bench_lane.py, A/B on one B200):
-                 * selects + predicated memory operations (no branch, no reconvergence point, no register shuffling
-                 * where the chains meet again) win without the recorder (+1 %) and with the order hash (+8 %); with the
-                 * recorder alone the two-branch form is 3.7 % faster (the predicated Sink block keeps more values live
-                 * across the staged stores). */
+                /* Two forms of the same updates, chosen per kernel by A/B measurement (tools/bench_lane.py, with
+                 * HS_LANE_PREDICATED=0/1 builds): selects + predicated memory operations (no branch, no reconvergence
+                 * point, no register shuffling where the chains meet again) won without the recorder and with the
+                 * order hash; with the recorder alone the two-branch form won (the predicated Sink block keeps more
+                 * values live across the staged stores). */
                 constexpr bool PREDICATED = HS_LANE_PREDICATED != 0 && (!(FLAGS & HS_LF_REC) || (FLAGS & HS_LF_HASH));
                 if (PREDICATED) {
                 const bool isC = !isA;

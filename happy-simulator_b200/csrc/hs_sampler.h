@@ -1,6 +1,6 @@
 /* hs_sampler.h -- counter-based RNG, natural log and int-ns/float-seconds time
  * arithmetic shared, from this ONE source, by
- *   - the sm_100a kernels (nvcc, __device__),
+ *   - the sm_90a kernels (nvcc, __device__),
  *   - the CPU oracle in oracle/ (gcc), and
  *   - the ctypes twins (hs_cpu_*) that the Philox plug-ins call when they are
  *     injected into the unmodified reference (tests/golden/gen_golden.py).

@@ -1,4 +1,4 @@
-/* hs_b200.h -- C-ABI of the B200 discrete-event engine (libhs_b200.so).
+/* hs_b200.h -- C-ABI of the H100 discrete-event engine (libhs_b200.so).
  *
  * The reference (adamfilli/happy-simulator) is pure Python and has NO FFI or
  * plugin registry for its run loop (SURVEY.md section 8(b)): the boundary it

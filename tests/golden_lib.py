@@ -1,12 +1,26 @@
 """Load the committed reference fixtures (tests/golden/*.npz)."""
 import glob
 import os
+import sys
 
 import numpy as np
 
 import happysim_b200 as hs
 
 GOLDEN_DIR = os.path.join(os.path.dirname(os.path.abspath(__file__)), "golden")
+# The unmodified reference (its package and examples) as build() installs it from the reference checkout
+# (oracle/Makefile, target `ref`); tests that need the reference's own classes import it from here.
+REF_DIR = os.path.join(os.path.dirname(os.path.dirname(os.path.abspath(__file__))), "oracle", "_ref")
+HAVE_REF = os.path.isdir(os.path.join(REF_DIR, "happysimulator"))
+NO_REF = "the reference is not installed in oracle/_ref (build() installs it when the reference checkout is present)"
+
+
+def import_reference():
+    """Put oracle/_ref on sys.path and return the reference's happysimulator package."""
+    if REF_DIR not in sys.path:
+        sys.path.insert(0, REF_DIR)
+    import happysimulator
+    return happysimulator
 
 
 def case_names(prefix):

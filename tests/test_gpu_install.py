@@ -1,25 +1,19 @@
 """install() on the GPU: an unchanged reference script, stock-seeded, prints the reference's own numbers.
-The reference travels to the GPU box as baseline/_ref (DESIGN.md section 8); skipped when it is absent."""
-import os
+Needs the reference as build() installs it into oracle/_ref; skipped when it is absent."""
 import random
-import sys
 
 import numpy as np
 import pytest
 
 pytestmark = pytest.mark.gpu
-ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
-REF = os.path.join(ROOT, "baseline", "_ref")
+import golden_lib as G
 
 
 @pytest.fixture(scope="module")
 def ref():
-    if not os.path.isdir(os.path.join(REF, "happysimulator")):
-        pytest.skip("baseline/_ref not installed")
-    if REF not in sys.path:
-        sys.path.insert(0, REF)
-    import happysimulator
-    return happysimulator
+    if not G.HAVE_REF:
+        pytest.skip(G.NO_REF)
+    return G.import_reference()
 
 
 def quickstart(ref, end_s=60.0, rate=8, n_servers=0):

@@ -1,6 +1,6 @@
 """happysim_b200.install(): the reference's own Simulation.run / ParallelRunner.run_replicas routed through the engine.
 
-CPU part (needs the reference importable: /root/reference in the build container or baseline/_ref): models that
+CPU part (needs the reference as build() installs it into oracle/_ref): models that
 do not lower fall through to the reference's Python loop unchanged; the example's user-defined step profile
 (examples/queuing/m_m_1_queue.py:104-169) tabulates exactly; eligibility rules.
 GPU part (tests/test_gpu_install.py): the stock-seeded README quick-start gives the reference's own numbers."""
@@ -12,24 +12,18 @@ import sys
 import numpy as np
 import pytest
 
-ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
-REF_DIRS = [os.path.join(ROOT, "baseline", "_ref"), "/root/reference"]
+import golden_lib as G
 
 
 def _reference():
-    for d in REF_DIRS:
-        if os.path.isdir(os.path.join(d, "happysimulator")):
-            if d not in sys.path:
-                sys.path.insert(0, d)
-            import happysimulator
-            return happysimulator
-    pytest.skip("reference not importable (baseline/_ref not installed)")
+    if not G.HAVE_REF:
+        pytest.skip(G.NO_REF)
+    return G.import_reference()
 
 
 def _example_module():
-    path = "/root/reference/examples/queuing/m_m_1_queue.py"
-    if not os.path.exists(path):
-        pytest.skip("reference examples live in /root/reference only (build container)")
+    _reference()
+    path = os.path.join(G.REF_DIR, "examples", "queuing", "m_m_1_queue.py")
     spec = importlib.util.spec_from_file_location("ref_example_mm1_t", path)
     mod = importlib.util.module_from_spec(spec)
     sys.modules["ref_example_mm1_t"] = mod

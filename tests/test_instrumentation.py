@@ -2,10 +2,10 @@
 and against hand-checked values."""
 import os
 import random
-import sys
 
-import pytest
+import numpy as np
 
+import golden_lib as G
 import happysim_b200 as hs
 
 
@@ -21,33 +21,47 @@ def test_data_aggregations_hand_checked():
     assert hs.Data().mean() == 0.0 and hs.Data().percentile(0.9) == 0.0 and not hs.Data()
 
 
-@pytest.mark.skipif(not os.path.isdir("/root/reference/happysimulator"), reason="reference checkout not present")
-def test_data_matches_the_reference_class():
-    sys.path.insert(0, "/root/reference")
-    from happysimulator.instrumentation.data import Data as RefData
+DATA_PERCENTILES = (0.0, 0.5, 0.9, 0.99, 1.0)
+HELPER_SIZES = (0, 1, 2, 3, 7, 100, 1001)
+
+
+def data_samples():
     rnd = random.Random(3)
-    samples = sorted((rnd.random() * 30, rnd.expovariate(2.0)) for _ in range(2000))
-    a, b = hs.Data(), RefData()
-    a._samples, b._samples = list(samples), list(samples)
-    for f in ("mean", "min", "max", "count", "sum", "std"):
-        assert getattr(a, f)() == getattr(b, f)()
-    for p in (0.0, 0.5, 0.9, 0.99, 1.0):
-        assert a.percentile(p) == b.percentile(p)
-    assert a.bucket(2.5).to_dict() == b.bucket(2.5).to_dict()
-    assert a.rate(5.0).values == b.rate(5.0).values
+    return sorted((rnd.random() * 30, rnd.expovariate(2.0)) for _ in range(2000))
+
+
+def helper_cases():
+    rnd = random.Random(1)
+    cases = []
+    for n in HELPER_SIZES:
+        v = sorted(rnd.random() * 10 for _ in range(n))
+        cases += [(v, p) for p in (-1, 0, 1e-9, 0.25, 0.5, 0.99, 0.999, 1, 2, rnd.random(), rnd.random())]
+    return cases
+
+
+def _reference_answers():
+    """What the reference's Data class and _percentile_sorted answered for these inputs
+    (tests/golden/gen_instrumentation_golden.py)."""
+    return np.load(os.path.join(G.GOLDEN_DIR, "instrumentation_data.npz"))
+
+
+def test_data_matches_the_reference_class():
+    want = _reference_answers()
+    a = hs.Data()
+    a._samples = data_samples()
+    assert [a.mean(), a.min(), a.max(), a.count(), a.sum(), a.std()] == want["stats"].tolist()
+    assert [a.percentile(p) for p in DATA_PERCENTILES] == want["percentiles"].tolist()
+    got = a.bucket(2.5).to_dict()
+    assert sorted(got) == sorted(k[len("bucket_"):] for k in want.files if k.startswith("bucket_"))
+    for k, v in got.items():
+        assert [float(x) for x in v] == want["bucket_" + k].tolist(), k
+    assert [list(r) for r in a.rate(5.0).values] == want["rate"].tolist()
 
 
 def test_percentile_helper_equals_the_reference_helper_float_for_float():
-    import random
-    import sys
-    import pytest
-    for d in ("/root/reference", __import__("os").path.join(__import__("os").path.dirname(__import__("os").path.dirname(__import__("os").path.abspath(__file__))), "baseline", "_ref")):
-        if __import__("os").path.isdir(__import__("os").path.join(d, "happysimulator")) and d not in sys.path:
-            sys.path.insert(0, d)
-    ref = pytest.importorskip("happysimulator.instrumentation.data")
     from happysim_b200.instrumentation import _percentile_sorted as mine
-    rnd = random.Random(1)
-    for n in (0, 1, 2, 3, 7, 100, 1001):
-        v = sorted(rnd.random() * 10 for _ in range(n))
-        for p in (-1, 0, 1e-9, 0.25, 0.5, 0.99, 0.999, 1, 2, rnd.random(), rnd.random()):
-            assert mine(v, p) == ref._percentile_sorted(v, p), (n, p)
+    cases = helper_cases()
+    want = _reference_answers()["helper"].tolist()
+    assert len(cases) == len(want)
+    for (v, p), w in zip(cases, want):
+        assert mine(v, p) == w, (len(v), p)

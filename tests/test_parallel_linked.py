@@ -74,10 +74,9 @@ def test_declaration_errors_follow_the_reference():
         hs.ParallelSimulation(parts, duration=1.0, links=[link])
 
 
-@pytest.mark.skipif(not __import__("os").path.isdir("/root/reference/happysimulator"), reason="reference checkout not present")
+@pytest.mark.skipif(not G.HAVE_REF, reason=G.NO_REF)
 def test_the_references_own_objects_lower_the_same_way():
-    import sys
-    sys.path.insert(0, "/root/reference")
+    G.import_reference()
     from happysimulator.components.common import Sink
     from happysimulator.components.server.server import Server
     from happysimulator.distributions.constant import ConstantLatency

@@ -1,7 +1,7 @@
 #!/bin/bash
 # A/B of thread-engine library variants on one GPU box: tools/ab_thread.sh <variant> ...   (libhs_<variant>.so, built with HS_B200_DEFS)
-cd "${GRAFT_REPO_ROOT:-$(dirname "$0")/..}"
-mkdir -p gpurun_out
+cd "$(dirname "$0")/.."
+OUT="${HS_OUT_DIR:-${TMPDIR:-/tmp}/hs_gpu_out}"; mkdir -p "$OUT"
 for v in "$@"; do
   HS_B200_LIB=$PWD/happy-simulator_b200/libhs_$v.so timeout 300 python tools/bench_thread.py
-done 2>&1 | tee gpurun_out/ab_thread.txt
+done 2>&1 | tee "$OUT"/ab_thread.txt

@@ -1,6 +1,6 @@
 """Summarise one kernel of an .ncu-rep into the text kept under profiles/:
-    python tools/ncu_summary.py gpurun_out/x.ncu-rep "header line" > profiles/rNN_x.txt
-(ncu --set full --clock-control none capture; metric names from /opt/skills/guides/B200_PROFILING.md)"""
+    python tools/ncu_summary.py x.ncu-rep "header line" > profiles/rNN_x.txt
+(ncu --set full --clock-control none capture)"""
 import csv, subprocess, sys
 
 KEEP = ("gpu__time_duration.sum", "dram__bytes_read.sum", "dram__bytes_write.sum",

@@ -1,5 +1,5 @@
 """Instruction-mnemonic counts per kernel of libhs_b200.so (cuobjdump -sass): the evidence for which memory paths a
-kernel uses -- STG.E.*.256 (256-bit sector stores, sm_100a), LDGSTS (cp.async), UBLKCP (TMA bulk copy), SYNCS (mbarrier),
+kernel uses -- STG.E.128 (the halves of the 32-byte sector stores), LDGSTS (cp.async), UBLKCP (TMA bulk copy), SYNCS (mbarrier),
 SHFL (warp shuffles), REDG/ATOMG, MUFU, DFMA ...      python tools/sass_counts.py > profiles/rNN_sass_counts.txt"""
 import collections, os, re, subprocess, sys
 ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
@@ -19,7 +19,7 @@ for line in out.splitlines():
             cnt[cur][op] += 1
 KEYS = ["STG.E.NA.EFL2.256", "STG.E.ENL2.256", "STG.E.128", "STG.E.64", "STG.E", "LDG.E.128", "LDG.E.64", "LDG.E", "LDGSTS.E.128", "LDGSTS",
         "UBLKCP", "CCTL.E.PF1", "SYNCS", "SHFL", "REDG", "ATOMG", "STS.128", "LDS.128", "DFMA", "DMUL", "DADD", "MUFU", "IMAD", "BRA", "BSSY"]
-print(f"# {os.path.relpath(lib, ROOT)}: SASS mnemonic counts per kernel (cuobjdump -sass, sm_100a)")
+print(f"# {os.path.relpath(lib, ROOT)}: SASS mnemonic counts per kernel (cuobjdump -sass, sm_90a)")
 for fn in sorted(cnt):
     if "hs_" not in fn:
         continue
