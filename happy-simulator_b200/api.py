@@ -680,15 +680,7 @@ class Simulation:
 
     # -- single run -------------------------------------------------------------
     def _rate_bound(self) -> float:
-        ents = self.model.entities
-        rate = 0.0
-        for i in self.model.ids_of(A.HS_ENT_SOURCE):
-            pi = int(ents["i3"][i])
-            if pi == 0:
-                rate += float(ents["d0"][i])
-            else:        # non-constant profile: bound by its largest rate
-                rate += lowering.profile_max_rate(self.model.profiles[pi - 1], self.model.profile_table)
-        return rate
+        return lowering.source_rate_bound(self.model)
 
     def _caps(self, n_hint: int | None = None):
         dur = self._end_time.to_seconds()

@@ -449,7 +449,6 @@ static int hs_warp_launch(hs_engine *E, const hs_run_params *p, uint32_t ring, b
 #define HS_LAUNCH_THREAD(F) case F: hs_thread_kernel<F><<<tblocks, HS_THREAD_BLOCK, dyn_smem, E->stream>>>(M, R, (unsigned char *)E->d_state.p, (hs_wring_entry *)E->d_rings.p, O); break;
 #define HS_LAUNCH_THREAD_WIDE(F) case F: hs_thread_kernel_wide<F><<<tblocks, HS_THREAD_BLOCK, dyn_smem, E->stream>>>(M, R, (unsigned char *)E->d_state.p, (hs_wring_entry *)E->d_rings.p, O); break;
         const bool linked_model = E->outbox_cap || E->inbox_cap || R.linked;
-        if (linked_model && (fl & HS_WF_PROFILE)) return fail(HS_ERR_INVALID, "linked partitions with non-constant rate profiles are not compiled in");
         /* small launches (every block resident at 4 blocks per SM, no shared-memory heap top, not linked): the spill-free
          * instantiation, see hs_thread_kernel_wide; HS_THREAD_WIDE=0/1 overrides (experiments) */
         bool wide = !R.heap_top && !linked_model && tblocks <= E->sm_count * HS_T_WIDE_BLOCKS;
@@ -466,8 +465,10 @@ static int hs_warp_launch(hs_engine *E, const hs_run_params *p, uint32_t ring, b
         HS_LAUNCH_THREAD(4) HS_LAUNCH_THREAD(5) HS_LAUNCH_THREAD(6) HS_LAUNCH_THREAD(7)
         HS_LAUNCH_THREAD(8) HS_LAUNCH_THREAD(9) HS_LAUNCH_THREAD(10) HS_LAUNCH_THREAD(11)
         HS_LAUNCH_THREAD(12) HS_LAUNCH_THREAD(13) HS_LAUNCH_THREAD(14) HS_LAUNCH_THREAD(15)
-        HS_LAUNCH_THREAD(16) HS_LAUNCH_THREAD(17) HS_LAUNCH_THREAD(18) HS_LAUNCH_THREAD(19)        /* LINKED (no PROFILE) */
+        HS_LAUNCH_THREAD(16) HS_LAUNCH_THREAD(17) HS_LAUNCH_THREAD(18) HS_LAUNCH_THREAD(19)        /* LINKED */
+        HS_LAUNCH_THREAD(20) HS_LAUNCH_THREAD(21) HS_LAUNCH_THREAD(22) HS_LAUNCH_THREAD(23)
         HS_LAUNCH_THREAD(24) HS_LAUNCH_THREAD(25) HS_LAUNCH_THREAD(26) HS_LAUNCH_THREAD(27)
+        HS_LAUNCH_THREAD(28) HS_LAUNCH_THREAD(29) HS_LAUNCH_THREAD(30) HS_LAUNCH_THREAD(31)
         default: return fail(HS_ERR_STATE, "no thread kernel for flags %d", fl);
         }
 #undef HS_LAUNCH_THREAD

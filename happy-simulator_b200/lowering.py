@@ -135,6 +135,20 @@ def profile_max_rate(pr, tables=None) -> float:
     return float(max(pr["p"][0:2]))
 
 
+def source_rate_bound(model) -> float:
+    """Sum over ``model``'s SOURCE rows of the largest rate each can reach: ``d0`` for a constant rate, the
+    profile's peak (``profile_max_rate``) otherwise -- a profile source is lowered with d0 = 0 (buffer sizing only)."""
+    ents = model.entities
+    rate = 0.0
+    for i in model.ids_of(A.HS_ENT_SOURCE):
+        pi = int(ents["i3"][i])
+        if pi == 0:
+            rate += float(ents["d0"][i])
+        else:
+            rate += profile_max_rate(model.profiles[pi - 1], model.profile_table)
+    return rate
+
+
 class _Seconds:
     """Stand-in for an Instant when probing a user's Profile.get_rate: the reference evaluates
     ``profile.get_rate(Instant.from_seconds(t))`` and profiles read ``time.to_seconds()`` (load/profile.py:37-110),

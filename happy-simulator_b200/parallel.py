@@ -69,13 +69,47 @@ class ParallelSimulationSummary:
     coordination_efficiency: float = 1.0
 
 
-def _events_bound(model, end_ns: int) -> float:
-    """Upper estimate of the Sink samples / service starts one replica of ``model`` produces (ring sizing)."""
-    from . import _abi as A
-    rate = 0.0
-    for i in model.ids_of(A.HS_ENT_SOURCE):
-        rate += float(model.entities["d0"][i])
-    return (rate * 4 + 50.0) * (end_ns / 1e9 + 1.0) + 4.0 * max(model.inbox_cap, 0)
+def _reaching_rates(lm) -> list[float]:
+    """Per partition of a LinkedModel: the summed peak rate of every source whose requests can reach it -- its own
+    and those of every partition upstream of it over links, followed transitively."""
+    from .lowering import source_rate_bound
+    own = [source_rate_bound(m) for m in lm.models]
+    upstream: list[set[int]] = [set() for _ in lm.models]
+    for p, ls in enumerate(lm.links):
+        for l in ls:
+            upstream[l.dest].add(p)
+    rates = []
+    for q in range(lm.n_partitions):
+        seen, todo = {q}, [q]
+        while todo:
+            for p in upstream[todo.pop()] - seen:
+                seen.add(p)
+                todo.append(p)
+        rates.append(sum(own[p] for p in seen))
+    return rates
+
+
+def _events_bound(rate: float, inbox_cap: int, end_ns: int) -> float:
+    """First estimate of the Sink samples / service starts one replica of a partition produces (ring sizing):
+    ``rate`` is the partition's entry of ``_reaching_rates``.  _run_linked checks the counts against it after the run."""
+    return (rate * 4 + 50.0) * (end_ns / 1e9 + 1.0) + 4.0 * max(inbox_cap, 0)
+
+
+_RINGS = (("sample_cap", "n_sink_samples", "Sink sample"), ("service_cap", "n_service_samples", "service time"),
+          ("record_cap", "events_processed", "event record"))
+
+
+def _short_rings(outs, caps) -> list[tuple[int, str, int]]:
+    """(partition, cap name, largest count over the replicas) of every recorder ring a linked run wrapped.  A record
+    ring of 0 slots is not in use (the partition's samples need no split by entity)."""
+    short = []
+    for q, (o, c) in enumerate(zip(outs, caps)):
+        s = o["summaries"]
+        for cap, count, _ in _RINGS:
+            n = int(s[count].max()) if len(s) else 0
+            if (cap != "record_cap" or c[cap]) and n > c[cap]:
+                short.append((q, cap, n))
+    return short
 
 
 class ParallelSimulation:
@@ -205,26 +239,43 @@ class ParallelSimulation:
         run = LinkedRun(lm, device=self._device)
         try:
             caps = []
-            for m in lm.models:
-                ev = max(64, int(_events_bound(m, self._end_ns)))
+            for m, rate in zip(lm.models, _reaching_rates(lm)):
+                ev = max(64, int(_events_bound(rate, m.inbox_cap, self._end_ns)))
                 many = len(m.ids_of(A.HS_ENT_SINK)) + len(m.ids_of(A.HS_ENT_PROBE)) > 1 or len(m.ids_of(A.HS_ENT_SERVER)) > 1
                 caps.append(dict(sample_cap=ev, service_cap=ev, record_cap=8 * ev if many else 0))   # records tell the sinks / servers apart
             # The reference's queues are unbounded, the device's are rings: a replica whose ring filled up stopped early
-            # (HS_ST_QUEUE_OVERFLOW).  Like Simulation.run(), grow the ring and run the whole thing again (every window
-            # starts from scratch: resume = 0 at window 0, a fresh coordinator) instead of handing that to the caller.
+            # (HS_ST_QUEUE_OVERFLOW).  A recorder ring that was too small wrapped: it holds only the last `cap` items,
+            # and a wrapped record ring credits samples to the wrong sink / server.  Like Simulation.run(), grow what was
+            # too small and run the whole thing again (every window starts from scratch: resume = 0 at window 0, a fresh
+            # coordinator) instead of handing that to the caller.  Growth happens before an attempt, so `ring` and
+            # `caps` are always what the last attempt ran with.
             ring = int(getattr(self, "queue_ring", 0) or 0)
-            for _attempt in range(6):
+            queue_full, short = False, []
+            for attempt in range(6):
+                if queue_full:
+                    ring = max(512, 4 * ring)
+                for q, cap, n in short:
+                    caps[q][cap] = 2 * n + 64
                 outs, (delivered, lost, over) = run.run(seed=self._seed, end_ns=self._end_ns, n_replicas=n_replicas,
                                                         replica_index_base=replica_index_base, caps=caps, flags=0, queue_ring=ring)
                 status = 0
                 for o in outs:
                     status |= int(np.bitwise_or.reduce(o["summaries"]["status"])) if len(o["summaries"]) else 0
-                if not (status & A.HS_ST_QUEUE_OVERFLOW) or (status & ~(A.HS_ST_QUEUE_OVERFLOW | A.HS_ST_LINK_TIE)) or over.any():
+                clean = not (status & ~A.HS_ST_LINK_TIE) and not over.any()
+                queue_full = bool(status & A.HS_ST_QUEUE_OVERFLOW and not (status & ~(A.HS_ST_QUEUE_OVERFLOW | A.HS_ST_LINK_TIE))
+                                  and not over.any())
+                short = _short_rings(outs, caps) if clean else []     # counts of a run that stopped early mean nothing
+                if not (queue_full or short):
                     break
-                ring = max(512, 4 * ring)
             self.last_queue_ring = ring
         finally:
             run.close()
+        if short:
+            q, cap, n = short[0]
+            what = next(w for c, _, w in _RINGS if c == cap)
+            raise RuntimeError(f"linked run: partition '{lm.names[q]}' recorded {n} items into its {what} ring of "
+                               f"{caps[q][cap]} device slots ({cap}) in the last of {attempt + 1} attempts; the ring "
+                               "wrapped, so its results are not published")
         wall = _time.monotonic() - t0
         bad = [(lm.names[q], int(s)) for q, o in enumerate(outs) for s in o["summaries"]["status"] if int(s) & ~A.HS_ST_LINK_TIE]
         if bad or over.any():

@@ -3,6 +3,7 @@ ParallelSimulation + WindowedCoordinator (parallel/simulation.py, parallel/coord
 the Philox streams injected as in gen_golden.py (ref_harness.run_reference_linked).
 
     python tests/golden/gen_linked_golden.py        # needs /root/reference; writes tests/golden/linked_*.npz
+    python tests/golden/gen_linked_golden.py tandem_heavy     # only the cases whose name contains the argument
 
 Per case: the partition models, the link table, and per partition the reference's summaries, entity statistics, event
 records, Sink samples and service times; plus the coordinator's window and cross-partition event counts."""
@@ -37,6 +38,24 @@ def tandem_over_a_link(loss=0.0, kind=CONST, latency=0.05):
     b.set_target(sb, snk)
     mb = b.build(); mb.inbox_cap = 64
     return LinkedModel([ma, mb], ["A", "B"], [[LinkSpec(1, kind, latency, loss, 0)], []], window_s=0.05)
+
+
+def tandem_heavy():
+    """A: Source(500/s) -> Server(c=4, exp 1 ms) -> [50 ms link] -> B: Server(c=4, exp 2 ms) -> Sink over 10 s: about
+    5 000 Sink samples in B, far more than the recorder rings of the light tandem hold.  The boxes are
+    ParallelSimulation.link_buffer wide, as the API lowers this declaration (tests/test_linked_volume.py)."""
+    a = hs.ModelBuilder()
+    src = a.source(rate=500.0)
+    sa = a.server("A.server", concurrency=4, mean_service_s=0.001)
+    rem = a.remote("B.server@A", link=0, dest_entity=0)
+    a.set_target(src, sa); a.set_target(sa, rem)
+    ma = a.build(); ma.outbox_cap = 256
+    b = hs.ModelBuilder()
+    sb = b.server("B.server", concurrency=4, mean_service_s=0.002)
+    snk = b.sink("B.sink")
+    b.set_target(sb, snk)
+    mb = b.build(); mb.inbox_cap = 256
+    return LinkedModel([ma, mb], ["A", "B"], [[LinkSpec(1, CONST, 0.05, 0.0, 0)], []], window_s=0.05)
 
 
 def aligned_ring(pumps=False):
@@ -106,6 +125,7 @@ def cases():
         "aligned_ring": (aligned_ring(), dict(seed=1, end_s=1.5)),
         "aligned_ring_spread": (aligned_ring(pumps=True), dict(seed=1, end_s=1.5)),
         "lossy_fanout": (lossy_fanout(), dict(seed=11, end_s=3.0)),
+        "tandem_heavy": (tandem_heavy(), dict(seed=5, end_s=10.0)),
     }
 
 

@@ -148,6 +148,40 @@ def oracle_run_linked(lm, params: list, *, end_ns, cseed, cseed_stride=0, crid_b
     return [b for b, _ in outs], delivered, lost, ends
 
 
+class OracleLinkedRun:
+    """``happysim_b200.linked.LinkedRun`` on the CPU oracle, same interface: install it with
+    ``monkeypatch.setattr(linked, "LinkedRun", OracleLinkedRun)`` and ParallelSimulation's whole host path (lowering,
+    ring sizing, the retry loop, the summary, the write-back) runs without a GPU.  Replica r of partition q draws from
+    the replica word ``q + g * (P + 1)``, the coordinator from ``P + g * (P + 1)``, exactly as on the device, and the
+    recorder rings are the ``caps`` passed in: a ring that is too small wraps as the device's does.
+
+    The oracle's queues are unbounded (hs_oracle.c never reads ``queue_ring`` and never sets HS_ST_QUEUE_OVERFLOW), so
+    this stand-in never reports a queue overflow and ``overflowed`` is all zeros.  ``calls`` keeps the keyword
+    arguments of every ``run``."""
+
+    def __init__(self, lm, *, device=0):
+        lm.validate()
+        self.lm, self.device = lm, device
+        self.windows = 0
+        self.calls = []
+
+    def close(self):
+        pass
+
+    def run(self, *, seed, end_ns, n_replicas=1, replica_index_base=0, caps=None, flags=A.HS_RUN_ORDER_HASH, queue_ring=0):
+        nP = self.lm.n_partitions
+        caps = caps or {}
+        per = [dict(caps[q] if isinstance(caps, (list, tuple)) else caps) for q in range(nP)]
+        self.calls.append(dict(seed=seed, end_ns=end_ns, n_replicas=n_replicas, replica_index_base=replica_index_base,
+                               caps=[dict(c) for c in per], flags=flags, queue_ring=queue_ring))
+        ps = [make_params(seed=seed, end_ns=end_ns, n_replicas=n_replicas, rid_base=q, rid_stride=nP + 1,
+                          replica_index_base=replica_index_base, queue_ring=queue_ring, flags=flags, **per[q])
+              for q in range(nP)]
+        outs, delivered, lost, ends = oracle_run_linked(self.lm, ps, end_ns=end_ns, cseed=seed)
+        self.windows = len(ends)
+        return outs, (delivered, lost, np.zeros(n_replicas, np.uint64))
+
+
 def oracle_run_trace(model, p: A.RunParams, targets, service):
     """One replica fed with externally captured draws (the reference's stock RNG outputs)."""
     d = model.desc()

@@ -125,6 +125,48 @@ def test_api_parallel_simulation_with_a_link_equals_the_reference_fixture():
     assert int(ens["B"]["summaries"]["events_processed"][0]) == int(z["p1_summaries"]["events_processed"][0])
 
 
+def test_api_tandem_heavy_equals_the_reference_fixture():
+    """The 500 req/s tandem (fixture linked_tandem_heavy, ~5 000 Sink samples in B) through hs.ParallelSimulation on
+    the device: the unmodified reference's lists, in full, on the script's own objects."""
+    import test_linked_volume as V
+    ps, parts = V.build("tandem_heavy")
+    summ = ps.run()
+    lm, kw, z = G.load_linked("linked_tandem_heavy")
+    (sa,), (sb, sink) = parts[0].entities, parts[1].entities
+    assert summ.total_windows == int(z["total_windows"]) and summ.total_cross_partition_events == int(z["cross_events"])
+    assert [s.total_events_processed for s in summ.partitions.values()] == [int(z[f"p{q}_summaries"]["events_processed"][0]) for q in range(2)]
+    assert len(sink.latencies_s) == len(z["p1_sink_samples"]) > 4000
+    assert sink.latencies_s == [float(x) for x in z["p1_sink_samples"]["latency_s"]]
+    assert [t.nanoseconds for t in sink.completion_times] == [int(x) for x in z["p1_sink_samples"]["completion_ns"]]
+    assert sb._service_times == [float(x) for x in z["p1_service_samples"]]
+    assert sa._service_times == [float(x) for x in z["p0_service_samples"]]
+    assert sink.events_received == int(z["p1_entity_stats"][0][1]["c0"]) and ps.link_ties == 0
+
+
+@pytest.mark.parametrize("name", ["tandem_heavy", "fan_in", "two_sinks", "chain", "profile_source"])
+def test_linked_volume_cases_on_the_device(name):
+    """The volume cases of tests/test_linked_volume.py through the real LinkedRun: the thread engine's linked runs with
+    inboxes of tens to hundreds of events per window and recorder rings of thousands of items publish exactly the
+    unwrapped oracle run."""
+    import test_linked_volume as V
+    ps, _ = V.build(name)
+    summ = ps.run()
+    want, delivered, lost, ends = V.truth(ps._linked, seed=ps._seed, end_ns=ps._end_ns)
+    assert ps.link_ties == 0 and np.array_equal(ps.last_delivered, delivered) and np.array_equal(ps.last_lost, lost)
+    V.check_published(ps, summ, want, delivered, ends)
+
+
+def test_linked_volume_ensemble_on_the_device():
+    """run_ensemble(16) of the 500 req/s tandem: every replica's rings, unrolled, equal its unwrapped oracle run."""
+    import test_linked_volume as V
+    ps, _ = V.build("tandem_heavy")
+    n = 16
+    ens, delivered, lost = ps.run_ensemble(n)
+    want, wd, wl, _ = V.truth(ps._linked, seed=ps._seed, end_ns=ps._end_ns, n_replicas=n)
+    assert np.array_equal(delivered, wd) and np.array_equal(lost, wl)
+    V.check_ensemble(ps._linked, ens, want, n)
+
+
 def test_random_linked_models_on_the_device():
     """The 72 random linked ParallelSimulations (tests/random_models.random_linked_model; oracle == reference on all of
     them, tests/test_random_linked.py): 6 replicas each on the device against the oracle.  A replica in which a delivered

@@ -97,9 +97,10 @@ def test_the_references_own_objects_lower_the_same_way():
         assert ps._linked.models[q].entities.tobytes() == lm.models[q].entities.tobytes()
 
 
-def test_a_full_device_queue_ring_is_grown_and_the_linked_run_repeated(monkeypatch):
+def test_a_full_queue_ring_is_grown_the_run_repeated_and_the_last_ring_reported(monkeypatch):
     """The reference's queues are unbounded; a device queue ring that filled up (HS_ST_QUEUE_OVERFLOW) is not the
-    caller's problem: the whole linked run is repeated with a larger ring (host logic, no device: LinkedRun is stubbed)."""
+    caller's problem: the whole linked run is repeated with a larger ring (host logic, no device: LinkedRun is stubbed).
+    The stub returns whole summary records, as the engine does: a clean run's recorder-ring counts are checked too."""
     import numpy as np
     from happysim_b200 import linked as L, parallel as P
     rings = []
@@ -109,7 +110,7 @@ def test_a_full_device_queue_ring_is_grown_and_the_linked_run_repeated(monkeypat
             self.lm, self.windows = lm, 0
         def run(self, *, seed, end_ns, n_replicas=1, replica_index_base=0, caps=None, flags=0, queue_ring=0):
             rings.append(queue_ring)
-            st = np.zeros(n_replicas, dtype=[("status", "<u4")])
+            st = np.zeros(n_replicas, dtype=A.SUMMARY_DTYPE)
             if queue_ring < 2048:
                 st["status"][0] = A.HS_ST_QUEUE_OVERFLOW
             self.windows = 80
@@ -128,7 +129,14 @@ def test_a_full_device_queue_ring_is_grown_and_the_linked_run_repeated(monkeypat
     ps.queue_ring = 4096
     ps._run_linked(1)
     assert rings == [4096]
-    StubRun.run = lambda self, **kw: ([{"summaries": np.array([(A.HS_ST_QUEUE_OVERFLOW,)], dtype=[("status", "<u4")])} for _ in self.lm.models],
-                                      (np.zeros(1, np.uint64),) * 3)
-    with pytest.raises(RuntimeError, match="queue_ring"):
+    def always_full(self, *, queue_ring, **kw):
+        rings.append(queue_ring)
+        st = np.zeros(1, dtype=A.SUMMARY_DTYPE)
+        st["status"] = A.HS_ST_QUEUE_OVERFLOW
+        return [{"summaries": st.copy()} for _ in self.lm.models], (np.zeros(1, np.uint64),) * 3
+    StubRun.run = always_full
+    rings.clear()
+    # six attempts from 4096 slots, x4 each: the message and last_queue_ring name the ring the last attempt ran with
+    with pytest.raises(RuntimeError, match=r"outgrew 4194304 device slots \(ParallelSimulation.queue_ring\)"):
         ps._run_linked(1)
+    assert rings == [4096 * 4 ** k for k in range(6)] and ps.last_queue_ring == 4194304
