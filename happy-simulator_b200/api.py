@@ -24,6 +24,7 @@ import numpy as np
 from . import _abi as A
 from . import lowering
 from .engine import Engine, make_params
+from .results import EntitySummary, QueueStats, SimulationSummary, replica_summary, write_back  # noqa: F401
 
 default_seed = 0
 
@@ -571,41 +572,6 @@ class LoadBalancer(Entity):
                                  requests_forwarded=self._requests_forwarded)
 
 
-# ----------------------------------------------------------------------------- summary
-@dataclass
-class QueueStats:
-    """instrumentation/summary.py:14-20"""
-    peak_depth: int
-    total_accepted: int
-    total_dropped: int
-
-
-@dataclass
-class EntitySummary:
-    """instrumentation/summary.py:23-44"""
-    name: str
-    entity_type: str
-    events_handled: int
-    queue_stats: QueueStats | None = None
-
-
-@dataclass
-class SimulationSummary:
-    """instrumentation/summary.py:47-87"""
-    duration_s: float
-    total_events_processed: int
-    events_cancelled: int = 0
-    events_per_second: float = 0.0
-    wall_clock_seconds: float = 0.0
-    entities: dict[str, EntitySummary] = field(default_factory=dict)
-
-    def to_dict(self) -> dict[str, Any]:
-        return {"duration_s": self.duration_s, "total_events_processed": self.total_events_processed,
-                "events_cancelled": self.events_cancelled, "events_per_second": self.events_per_second,
-                "wall_clock_seconds": self.wall_clock_seconds,
-                "entities": {k: vars(v) for k, v in self.entities.items()}}
-
-
 def stock_streams(seed: int, n_replicas: int, n_draws: int, seed_stride: int = 1):
     """The reference's two process-global MT19937 streams as unit-rate exponential variates:
     row r is what ``random.seed(seed + r*seed_stride); numpy.random.seed(seed + r*seed_stride)`` yields.
@@ -642,7 +608,7 @@ class Simulation:
     def __init__(self, start_time: Instant | None = None, end_time: Instant | None = None, sources=None,
                  entities=None, probes=None, trace_recorder=None, fault_schedule=None, duration: float | None = None,
                  *, seed: int | None = None, replica: int = 0, device: int = 0, rng: str = "philox",
-                 queue_ring: int | None = None):
+                 queue_ring: int | None = None, _lowered: tuple | None = None):
         if duration is not None and end_time is not None:
             raise ValueError("Cannot specify both 'duration' and 'end_time'")
         if start_time is not None and start_time.nanoseconds != 0:
@@ -670,21 +636,27 @@ class Simulation:
         self._queue_ring = int(queue_ring) if queue_ring else 0
         self.last_run_info: dict = {}
         self._summary: SimulationSummary | None = None
-        self._instant_cls = Instant
-        self.model, self.objects = lowering.lower(self._sources, self._entities, probes=self._probes,
-                                                  horizon_s=self._end_time.to_seconds())
+        if _lowered is None:
+            _lowered = (*lowering.lower(self._sources, self._entities, probes=self._probes,
+                                        horizon_s=self._end_time.to_seconds()), Instant)
+        self.model, self.objects, self._instant_cls = _lowered
+
+    @classmethod
+    def _from_lowered(cls, model, objects, *, sources, entities, end_ns: int, seed: int | None = None, replica: int = 0,
+                      device: int = 0, instant_cls=Instant) -> "Simulation":
+        """A Simulation around a model lowered elsewhere, from a reference Simulation's object graph
+        (``run_lowered``, ``install()``); its results are published with ``instant_cls`` time points."""
+        return cls(end_time=Instant(int(end_ns)), sources=sources, entities=entities, seed=seed, replica=replica,
+                   device=device, _lowered=(model, objects, instant_cls))
 
     @property
     def summary(self):
         return self._summary
 
     # -- single run -------------------------------------------------------------
-    def _rate_bound(self) -> float:
-        return lowering.source_rate_bound(self.model)
-
     def _caps(self, n_hint: int | None = None):
         dur = self._end_time.to_seconds()
-        rate = self._rate_bound()
+        rate = lowering.source_rate_bound(self.model)
         req = int(rate * dur * 1.3 + 6 * math.sqrt(rate * dur + 1) + 64)
         n_srv = len(self.model.ids_of(A.HS_ENT_SERVER))
         chain = 1 if (n_srv <= 1 or self.model.ids_of(A.HS_ENT_LB)) else n_srv     # tandem: one start per stage
@@ -707,7 +679,7 @@ class Simulation:
         for i in self.model.ids_of(A.HS_ENT_SERVER):
             mean = float(ents["d0"][i])
             cap += (max(1, int(ents["i0"][i])) / mean) if mean > 0 else float("inf")
-        backlog = max(0.0, (self._rate_bound() - cap) * dur)
+        backlog = max(0.0, (lowering.source_rate_bound(self.model) - cap) * dur)
         ring = 256
         while ring < min(2.5 * backlog + 64, 1 << 22):
             ring *= 2
@@ -715,133 +687,6 @@ class Simulation:
 
     def run(self) -> SimulationSummary:
         return _run_many([self], seed=self._seed, seed_stride=0, rid_base=self._replica, rid_stride=0)[0]
-
-    def _write_back(self, out, r: int) -> None:
-        """Publish replica ``r`` onto the Python objects, where the reference's callers look."""
-        st = out["entity_stats"][r]
-        kinds = self.model.entities["kind"]
-        s = out["summaries"][r]
-        n_smp, n_svc = int(s["n_sink_samples"]), int(s["n_service_samples"])
-        samples = out["sink_samples"][r][:n_smp] if out.get("sink_samples") is not None else None
-        sinks = self.model.ids_of(A.HS_ENT_SINK) + self.model.ids_of(A.HS_ENT_PROBE)
-        servers = self.model.ids_of(A.HS_ENT_SERVER)
-        per_server = {i: [] for i in servers}
-        per_sink = {i: None for i in sinks}
-        if samples is not None:
-            if len(sinks) == 1:
-                per_sink[sinks[0]] = samples
-            elif out.get("records") is not None:
-                rec = out["records"][r][: int(s["events_processed"])]
-                who = rec["entity"][(rec["kind"] == A.HS_EV_REQ_SINK) | (rec["kind"] == A.HS_EV_PROBE)][: len(samples)]
-                for i in sinks:
-                    per_sink[i] = samples[who == i]
-        if out.get("service_samples") is not None:
-            svc = out["service_samples"][r][:n_svc]
-            if len(servers) == 1:
-                per_server[servers[0]] = [float(x) for x in svc]
-            elif out.get("records") is not None:
-                rec = out["records"][r][: int(s["events_processed"])]
-                who = rec["entity"][rec["kind"] == A.HS_EV_REQ_WORKER][: len(svc)]
-                for ent, x in zip(who, svc):
-                    per_server[int(ent)].append(float(x))
-        # Probe objects: their ticking is objects[i] (a SOURCE row); the measurement row it targets
-        # (kind PROBE, beyond len(objects)) carries the samples
-        for i, o in enumerate(self.objects):
-            if int(kinds[i]) == A.HS_ENT_SOURCE and hasattr(o, "data_sink"):
-                pid = int(self.model.entities["target"][i])
-                sm = per_sink.get(pid)
-                if sm is not None:
-                    o.data_sink._samples = [(float(int(t)) / 1_000_000_000, float(x))
-                                            for t, x in zip(sm["completion_ns"], sm["latency_s"])]
-        for i, o in enumerate(self.objects):
-            k = int(kinds[i])
-            row = st[i]
-            if k == A.HS_ENT_SOURCE:
-                o._generated_count = int(row["c0"])
-                if hasattr(o._event_provider, "_generated"):
-                    o._event_provider._generated = int(row["c1"])
-            elif k == A.HS_ENT_SERVER:
-                o._queue.stats_accepted, o._queue.stats_dropped = int(row["c0"]), int(row["c1"])
-                o._requests_completed, o._requests_rejected = int(row["c2"]), int(row["c3"])
-                o._total_service_time = float(row["f0"])
-                o._service_times = per_server[i]
-            elif k == A.HS_ENT_CACHE_SERVER:
-                o._queue.stats_accepted, o._queue.stats_dropped = int(row["c0"]), int(row["c1"])
-                o.stats.requests_processed, o.stats.cache_misses, o.stats.cache_hits = int(row["c2"]), int(row["c3"]), int(row["f0"])
-                if out.get("sketches") is not None:
-                    ins = self.model.cache_views(out["sketches"])[i][r]
-                    K = len(ins) - 1
-                    times = {("customer:unknown" if j == K else f"customer:{j}"): float(t) for j, t in enumerate(ins) if t != 0.0}
-                    if hasattr(o, "_insert_times"):
-                        o._insert_times = times
-                    elif getattr(o, "_eviction_policy", None) is not None:      # the example's own object, already initialised
-                        o._eviction_policy._insert_times = times
-            elif k == A.HS_ENT_SINK and hasattr(o, "data"):          # LatencyTracker / ThroughputTracker
-                o.count = int(row["c0"])
-                sm = per_sink[i]
-                if sm is not None:
-                    one = getattr(o, "_sample_value", None) == "one" or type(o).__name__ == "ThroughputTracker"
-                    o.data._samples = [(float(int(t)) / 1_000_000_000, 1.0 if one else float(x))
-                                       for t, x in zip(sm["completion_ns"], sm["latency_s"])]
-            elif k == A.HS_ENT_SINK:
-                o.events_received = int(row["c0"])
-                o._latency_sum = float(row["f0"])
-                sm = per_sink[i]
-                if sm is not None:
-                    o.completion_times = [self._instant_cls(int(t)) for t in sm["completion_ns"]]
-                    o.latencies_s = [float(x) for x in sm["latency_s"]]
-            elif k == A.HS_ENT_COUNTER:
-                o.total = int(row["c0"])
-                o.by_type = {"Request": o.total} if o.total else {}
-            elif k == A.HS_ENT_LB:
-                o._requests_received, o._requests_forwarded = int(row["c0"]), int(row["c1"])
-            elif k == A.HS_ENT_SKETCH:
-                o._events_processed = int(row["c0"])
-                sk = o._topk if hasattr(o, "_topk") else o._tdigest if hasattr(o, "_tdigest") else o._sketch
-                if out.get("sketches") is not None and hasattr(sk, "_load_device_state"):
-                    sk._load_device_state(self.model.sketch_views(out["sketches"])[i][r], int(row["c1"]))
-                elif out.get("sketches") is not None:      # a reference sketch object: fill its own fields
-                    state = self.model.sketch_views(out["sketches"])[i][r]
-                    algo = int(self.model.entities["i0"][i])
-                    if algo == A.HS_SK_HLL:
-                        sk._registers = [int(x) for x in state]
-                    elif algo == A.HS_SK_CMS:
-                        sk._counters = [[int(x) for x in rowc] for rowc in state]
-                    elif algo == A.HS_SK_BLOOM:
-                        sk._bits = [int(x) for x in state]
-                        sk._bits_set = sum(bin(w).count("1") for w in sk._bits)
-                    else:                                  # TopK / TDigest: rebuild the reference's own cells
-                        import sys as _sys
-                        from . import sketching as _sk
-                        mod = _sys.modules[type(sk).__module__]
-                        if algo == A.HS_SK_RESERVOIR:
-                            _sk.load_reservoir_state(sk, state)
-                        elif algo == A.HS_SK_TOPK:
-                            t = _sk.TopK(int(self.model.entities["i2"][i])); t._load_device_state(state, int(row["c1"]))
-                            sk._counters = {it: mod._Counter(item=it, count=c[0], error=c[1]) for it, c in t._counters.items()}
-                        else:
-                            d = _sk.TDigest(float(self.model.entities["d0"][i])); d._load_device_state(state)
-                            sk._centroids = [mod._Centroid(mean=m_, count=c_) for m_, c_ in zip(d._means, d._counts)]
-                            sk._buffer = list(d._buffer)
-                            sk._min_value, sk._max_value = d._min_value, d._max_value
-                    sk._total_count = int(row["c1"])
-
-    def _entity_summaries(self):
-        """core/simulation.py:560-591: only objects passed as entities=, events_handled from
-        count | events_received | stats_processed, queue stats for queued resources."""
-        res = {}
-        for o in self._entities:
-            qs = None
-            if hasattr(o, "_queue") and hasattr(o, "_concurrency_model"):
-                qs = QueueStats(peak_depth=0, total_accepted=o.stats_accepted, total_dropped=o.stats_dropped)
-            handled = 0
-            for attr in ("count", "events_received", "stats_processed"):
-                v = getattr(o, attr, None)
-                if isinstance(v, int):
-                    handled = v
-                    break
-            res[o.name] = EntitySummary(name=o.name, entity_type=type(o).__name__, events_handled=handled, queue_stats=qs)
-        return res
 
     # -- ensembles ----------------------------------------------------------------
     def run_ensemble(self, n_replicas: int, *, seed: int | None = None, seed_stride: int = 0, rid_base: int = 0,
@@ -1011,15 +856,10 @@ def _run_many(sims, *, seed: int, seed_stride: int, rid_base: int, rid_stride: i
     wall = _time.monotonic() - t0
     res = []
     for k, sm in enumerate(sims):
-        sm._write_back(out, k)
-        s = summ[k]
-        duration_s = float(int(s["final_time_ns"])) / 1_000_000_000
-        ev = int(s["events_processed"])
+        write_back(sm.model, sm.objects, out, k, sm._instant_cls)
         sm.last_run_info = {"launches": launches, "wall_s": wall, "queue_ring": ring, "batched_with": n,
-                            "device_ms_last_launch": eng.last_run_ms(), "status": int(s["status"])}
-        sm._summary = SimulationSummary(duration_s=duration_s, total_events_processed=ev, events_cancelled=0,
-                                        events_per_second=ev / duration_s if duration_s > 0 else 0.0,
-                                        wall_clock_seconds=wall, entities=sm._entity_summaries())
+                            "device_ms_last_launch": eng.last_run_ms(), "status": int(summ[k]["status"])}
+        sm._summary = replica_summary(summ[k], wall, sm._entities)
         res.append(sm._summary)
     return res
 
@@ -1047,19 +887,10 @@ def run_lowered(ref_sim, model=None, objects=None, *, seed: int | None = None, r
     if model is None:
         model, objects = lowering.lower(ref_sim._sources, ref_sim._entities, probes=getattr(ref_sim, "_probes", None) or None,
                                         horizon_s=float(int(ref_sim._end_time.nanoseconds)) / 1e9)
-    shell = Simulation.__new__(Simulation)
-    shell._start_time = Instant.Epoch
-    shell._end_time = Instant(int(ref_sim._end_time.nanoseconds))
-    shell._sources, shell._entities = list(ref_sim._sources), list(ref_sim._entities)
-    shell._seed = default_seed if seed is None else int(seed)
-    shell._replica, shell._device, shell._summary = int(replica), device, None
-    shell._rng, shell._queue_ring, shell.last_run_info = "philox", 0, {}
-    shell._probes = []
-    shell._instant_cls = type(ref_sim._start_time)
-    shell.model, shell.objects = model, objects
-    if trace_fn is not None:
-        return _run_many([shell], seed=shell._seed, seed_stride=0, rid_base=shell._replica, rid_stride=0, trace_fn=trace_fn)[0]
-    return shell.run()
+    sim = Simulation._from_lowered(model, objects, sources=ref_sim._sources, entities=ref_sim._entities,
+                                   end_ns=ref_sim._end_time.nanoseconds, seed=seed, replica=replica, device=device,
+                                   instant_cls=type(ref_sim._start_time))
+    return _run_many([sim], seed=sim._seed, seed_stride=0, rid_base=sim._replica, rid_stride=0, trace_fn=trace_fn)[0]
 
 
 # ----------------------------------------------------------------------------- parallel/runner.py
@@ -1092,14 +923,10 @@ class _ReplicaResults:
         return len(self.raw["summaries"])
 
     def _one(self, i: int) -> ParallelResult:
-        sim, out = self._sim, self.raw
-        sim._write_back(out, i)
-        s = out["summaries"][i]
-        d = float(int(s["final_time_ns"])) / 1_000_000_000
-        n = int(s["events_processed"])
-        return ParallelResult(name=f"replica_{i}", status=int(s["status"]), summary=SimulationSummary(
-            duration_s=d, total_events_processed=n, events_per_second=n / d if d > 0 else 0.0,
-            wall_clock_seconds=self._wall, entities=sim._entity_summaries()))
+        sim, s = self._sim, self.raw["summaries"][i]
+        write_back(sim.model, sim.objects, self.raw, i, sim._instant_cls)
+        return ParallelResult(name=f"replica_{i}", status=int(s["status"]),
+                              summary=replica_summary(s, self._wall, sim._entities))
 
     def __getitem__(self, i):
         if isinstance(i, slice):

@@ -157,29 +157,12 @@ def install(*, device: int = 0, verbose: bool = False) -> None:
             st["fallbacks"] += 1
             st["last_fallback_reason"] = str(e)
             return orig_replicas(self, build_fn, n_replicas, base_seed)
-        shell = api.Simulation.__new__(api.Simulation)
-        shell._start_time = api.Instant.Epoch
-        shell._end_time = api.Instant(int(ref_sim._end_time.nanoseconds))
-        shell._sources, shell._entities, shell._probes = list(ref_sim._sources), list(ref_sim._entities), []
-        shell._seed, shell._replica, shell._device, shell._summary = int(base_seed), 0, _state["device"], None
-        shell._rng, shell._queue_ring, shell.last_run_info = "philox", 0, {}
-        shell._instant_cls = type(ref_sim._start_time)
-        shell.model, shell.objects = model, objects
-        t0 = _time.monotonic()
-        out = shell.run_ensemble(n_replicas, seed=base_seed, seed_stride=1, rid_base=0, rid_stride=0,
-                                 queue_ring=shell._queue_ring_hint(), flags=0)
-        wall = _time.monotonic() - t0
+        sim = api.Simulation._from_lowered(model, objects, sources=ref_sim._sources, entities=ref_sim._entities,
+                                           end_ns=ref_sim._end_time.nanoseconds, seed=base_seed, device=_state["device"],
+                                           instant_cls=type(ref_sim._start_time))
+        res = api.ParallelRunner().run_replicas(lambda: sim, n_replicas, base_seed, flags=0)
         st["device_runs"] += 1
-        res = []
-        for i in range(n_replicas):
-            s = out["summaries"][i]
-            d = float(int(s["final_time_ns"])) / 1e9
-            ev = int(s["events_processed"])
-            shell._write_back(out, i)
-            res.append(R.ParallelResult(name=f"replica_{i}", summary=_to_ref_summary(api.SimulationSummary(
-                duration_s=d, total_events_processed=ev, events_per_second=ev / d if d > 0 else 0.0,
-                wall_clock_seconds=wall, entities=shell._entity_summaries()))))
-        return res
+        return [R.ParallelResult(name=r.name, summary=_to_ref_summary(r.summary)) for r in res]
 
     S.Simulation.__init__ = __init__
     S.Simulation.run = run

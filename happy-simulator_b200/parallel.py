@@ -13,8 +13,9 @@ import numpy as np
 from dataclasses import dataclass, field
 from typing import Any
 
-from .api import EntitySummary, Simulation, SimulationSummary
+from .api import Instant, Simulation
 from .lowering import UnsupportedModelError
+from .results import EntitySummary, SimulationSummary, replica_summary, write_back
 
 
 @dataclass
@@ -110,6 +111,17 @@ def _short_rings(outs, caps) -> list[tuple[int, str, int]]:
             if (cap != "record_cap" or c[cap]) and n > c[cap]:
                 short.append((q, cap, n))
     return short
+
+
+def _aggregate(summaries: dict[str, SimulationSummary]) -> dict:
+    """parallel/summary.py: total events, longest duration, events per second and merged entities of the partitions."""
+    total = sum(s.total_events_processed for s in summaries.values())
+    duration_s = max((s.duration_s for s in summaries.values()), default=0.0)
+    merged = {}
+    for s in summaries.values():
+        merged.update(s.entities)
+    return dict(duration_s=duration_s, total_events_processed=total,
+                events_per_second=total / duration_s if duration_s > 0 else 0.0, partitions=summaries, entities=merged)
 
 
 class ParallelSimulation:
@@ -303,28 +315,15 @@ class ParallelSimulation:
     def _summarise_linked(self, outs, delivered, lost, wall, windows) -> ParallelSimulationSummary:
         """coordinator.py:123-172: per-partition summaries from the partitions' final state, the aggregate like
         _build_summary; results are written back onto the script's own objects (replica 0)."""
-        from .api import Instant
         lm = self._linked
         summaries = {}
         for q, name in enumerate(lm.names):
-            shell = Simulation.__new__(Simulation)
-            shell.model, shell.objects, shell._instant_cls = lm.models[q], lm.objects[q], Instant
-            shell._entities = [o for o in self._partitions[q].entities if any(o is x for x in lm.objects[q])]
-            shell._write_back(outs[q], 0)
-            s = outs[q]["summaries"][0]
-            d = float(int(s["final_time_ns"])) / 1e9
-            ev = int(s["events_processed"])
-            summaries[name] = SimulationSummary(duration_s=d, total_events_processed=ev, events_per_second=ev / d if d > 0 else 0.0,
-                                                wall_clock_seconds=wall, entities=shell._entity_summaries())
-        total = sum(s.total_events_processed for s in summaries.values())
-        duration_s = max((s.duration_s for s in summaries.values()), default=0.0)
-        merged = {}
-        for s in summaries.values():
-            merged.update(s.entities)
+            write_back(lm.models[q], lm.objects[q], outs[q], 0, Instant)
+            entities = [o for o in self._partitions[q].entities if any(o is x for x in lm.objects[q])]
+            summaries[name] = replica_summary(outs[q]["summaries"][0], wall, entities)
         n = len(summaries)
         return ParallelSimulationSummary(
-            duration_s=duration_s, total_events_processed=total, events_per_second=total / duration_s if duration_s > 0 else 0.0,
-            wall_clock_seconds=wall, partitions=summaries, entities=merged,
+            **_aggregate(summaries), wall_clock_seconds=wall,
             partition_wall_times={nm: wall / n for nm in summaries}, speedup=1.0, parallelism_efficiency=1.0 / n if n else 1.0,
             total_windows=windows, total_cross_partition_events=int(delivered[0]), window_size_s=lm.window_s)
 
@@ -365,16 +364,9 @@ class ParallelSimulation:
                 walls[names[i]] = dt / len(g)
         summaries = {n: summaries[n] for n in names}
         wall = _time.monotonic() - t0
-        total = sum(s.total_events_processed for s in summaries.values())
-        duration_s = max((s.duration_s for s in summaries.values()), default=0.0)
-        merged = {}
-        for s in summaries.values():
-            merged.update(s.entities)
         seq = sum(walls.values())
         speedup = seq / wall if wall > 0 else 1.0
         n = len(summaries)
         return ParallelSimulationSummary(
-            duration_s=duration_s, total_events_processed=total,
-            events_per_second=total / duration_s if duration_s > 0 else 0.0, wall_clock_seconds=wall,
-            partitions=summaries, entities=merged, partition_wall_times=walls, speedup=speedup,
+            **_aggregate(summaries), wall_clock_seconds=wall, partition_wall_times=walls, speedup=speedup,
             parallelism_efficiency=speedup / n if n else 1.0)

@@ -9,6 +9,7 @@ import numpy as np
 
 import happysim_b200
 from happysim_b200 import _abi as A
+from happysim_b200.engine import make_params
 
 _ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
 _SO = os.path.join(_ROOT, "oracle", "libhs_oracle.so")
@@ -62,21 +63,6 @@ def lib():
         L.hs_sketch_layout.restype = C.c_int
         _lib = L
     return _lib
-
-
-def make_params(*, seed=1234, end_ns, n_replicas=1, seed_stride=0, rid_base=0, rid_stride=1,
-                replica_index_base=0, replicas_per_cell=1, record_cap=0, sample_cap=0, service_cap=0,
-                queue_ring=0, engine=0, window_end_ns=-1, resume=0,
-                flags=A.HS_RUN_ORDER_HASH, max_events=0) -> A.RunParams:
-    p = A.RunParams()
-    p.seed, p.seed_stride, p.rid_base, p.rid_stride = seed, seed_stride, rid_base, rid_stride
-    p.end_ns = int(end_ns)
-    p.n_replicas, p.replica_index_base, p.replicas_per_cell = n_replicas, replica_index_base, max(1, replicas_per_cell)
-    p.record_cap, p.sample_cap, p.service_cap = record_cap, sample_cap, service_cap
-    p.queue_ring, p.engine = queue_ring, engine
-    p.window_end_ns, p.resume, p.flags = int(window_end_ns), resume, flags
-    p.max_events = int(max_events)
-    return p
 
 
 def alloc_outputs(n_entities: int, p: A.RunParams, sketch_bytes: int = 0):

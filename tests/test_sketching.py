@@ -9,7 +9,7 @@ import pytest
 import golden_lib as G
 import happysim_b200 as hs
 import oracle_lib as O
-from happysim_b200 import _abi as A, distributed as D, engine, lowering
+from happysim_b200 import _abi as A, distributed as D, engine, lowering, results
 from happysim_b200.engine import EngineError
 
 
@@ -350,7 +350,7 @@ def test_hashed_on_the_device_rows_give_the_reference_states(name):
 
 
 def test_write_back_of_sketch_states_onto_the_mirror_objects():
-    """Simulation._write_back with oracle outputs standing in for the device's (same layout): the INTEGRATION.md
+    """results.write_back with oracle outputs standing in for the device's (same layout): the INTEGRATION.md
     example -- TopKCollector, QuantileEstimator, HyperLogLog collector behind a consistent-hash ring, Zipf ids."""
     top = hs.TopKCollector("heavy", k=10)
     p99 = hs.QuantileEstimator("lat", hs.LatencyExtractor(), compression=100)
@@ -362,7 +362,7 @@ def test_write_back_of_sketch_states_onto_the_mirror_objects():
     sim = hs.Simulation(end_time=hs.Instant.from_seconds(30), sources=[src], entities=[lb, *servers, top, p99, seen])
     engine.validate_model(sim.model)
     out = O.oracle_run(sim.model, O.make_params(seed=1, end_ns=30 * 10**9, n_replicas=2))
-    sim._write_back(out, 1)
+    results.write_back(sim.model, sim.objects, out, 1, hs.Instant)
     i_top, i_p99, i_seen = (sim.objects.index(o) for o in (top, p99, seen))
     st = out["entity_stats"][1]
     assert top.events_processed == int(st[i_top]["c0"]) == top.total_count > 500
