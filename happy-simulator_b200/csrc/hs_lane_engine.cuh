@@ -144,36 +144,15 @@ struct hs_lane_out {
     uint32_t *hist;                   /* [replica][HS_HIST_BINS] or NULL */
 };
 
-/* 256-bit global store: one full 32-byte sector per lane, written as two back-to-back 128-bit stores
- * (STG.E.128, the widest global store of sm_90a) to the two halves of the sector.  The recorder streams
- * are write-once per ring pass, so they are written with the streaming policy (st.global.cs,
- * HS_ST256_POLICY 2).  1 selects L1 no-allocate + an L2 evict-first cache policy, 0 the default
- * write-back policy; kept as a compile-time switch for A/B measurements.  tools/bench_lane.py on one
- * H100 80GB HBM3 (400 W power limit), record mode, 65 536 replicas: 2 -> 37.1e9, 1 -> 35.3e9,
- * 0 -> 32.2e9 events/s (profiles/h100_lane_store_policy_ab.txt). */
-#ifndef HS_ST256_POLICY
-#define HS_ST256_POLICY 2
-#endif
 #ifndef HS_LANE_PREDICATED
 #define HS_LANE_PREDICATED 1    /* SIMPLE chains: state updates as selects + predicated memory operations (0: two branches) */
 #endif
-__device__ __forceinline__ void hs_st128(void *p, const uint4 a)
-{
-#if HS_ST256_POLICY == 1
-    asm volatile("{\n\t.reg .b64 pol;\n\t"
-                 "createpolicy.fractional.L2::evict_first.b64 pol, 1.0;\n\t"
-                 "st.global.L1::no_allocate.L2::cache_hint.v4.b32 [%0], {%1,%2,%3,%4}, pol;\n\t}"
-#elif HS_ST256_POLICY == 2
-    asm volatile("st.global.cs.v4.b32 [%0], {%1,%2,%3,%4};"
-#else
-    asm volatile("st.global.v4.b32 [%0], {%1,%2,%3,%4};"
-#endif
-                 :: "l"(p), "r"(a.x), "r"(a.y), "r"(a.z), "r"(a.w) : "memory");
-}
+/* one full 32-byte sector per lane, as two back-to-back streaming 128-bit stores (STG.E.128, the widest
+ * global store of sm_90a): the recorder streams are write-once per ring pass */
 __device__ __forceinline__ void hs_st256(void *p, const uint4 a, const uint4 b)
 {
-    hs_st128(p, a);
-    hs_st128((uint4 *)p + 1, b);
+    __stcs((uint4 *)p, a);
+    __stcs((uint4 *)p + 1, b);
 }
 
 /* next arrival of a constant-rate profile, with the reference's "time travel" outcome
@@ -200,11 +179,10 @@ hs_lane_kernel(hs_lane_model M, hs_lane_run P, hs_lane_state *__restrict__ state
     constexpr uint32_t STAGE_ROWS = (FLAGS & HS_LF_REC) ? HS_STAGE : 1;
     __shared__ int64_t sh_t[HS_DRAW_BUF][HS_LANE_THREADS];       /* arrival times A_k (ns)          */
     __shared__ double sh_svc[HS_DRAW_BUF][HS_LANE_THREADS];      /* service: Duration.to_seconds()  */
-    /* recorder staging, [slot][lane]: a lane only ever touches its own 16-byte column, so neither the
-     * per-event writes nor the flush reads conflict, whatever slot each lane is at.  A lane that holds a
-     * full 128-byte group (8 records) writes it itself as four 256-bit stores (whole 32-byte sectors,
-     * the four sectors of one line back to back).  Sink samples (16 B) and service times (8 B) are paired /
-     * quadrupled the same way into one 32-byte sector per store. */
+    /* recorder staging, [slot][lane]: a lane writes only its own 16-byte column, so the per-event writes do
+     * not conflict, whatever slot each lane is at.  Full 128-byte groups (8 records) are written by the whole
+     * warp, whole lines per store (the flush at the top of the loop).  Sink samples (16 B) and service
+     * times (8 B) are paired / quadrupled into one 32-byte sector per lane and store. */
     __shared__ __align__(16) uint4 sh_rec[STAGE_ROWS][HS_LANE_THREADS];
     __shared__ __align__(16) uint4 sh_smp[(FLAGS & HS_LF_REC) ? HS_LANE_THREADS : 1];        /* first Sink sample of a pair */
     __shared__ double sh_sv[(FLAGS & HS_LF_REC) ? 3 : 1][HS_LANE_THREADS];                   /* first three service times of a quad */
@@ -529,26 +507,51 @@ hs_lane_kernel(hs_lane_model M, hs_lane_run P, hs_lane_state *__restrict__ state
         const unsigned todo = __ballot_sync(0xffffffffu, !finished);
         if (todo == 0u) break;
         if (__any_sync(0xffffffffu, need)) HS_REFILL_ROUND();
-        /* SIMPLE: the three shared-memory operands of the next chain are requested first, so their
-         * latency is covered by the flush below: next arrival time, next service time, queue head */
+        if ((FLAGS & HS_LF_REC) && staged) {
+            /* the warp writes the full 128-byte groups of all its lanes together, four whole lines per store
+             * instruction: lane l moves record l / 4 of the group of the (l % 4)-th owner of the round (so a
+             * quarter-warp reads two rows of four staging columns).  An owner's group is rows 0-7 or 8-15 of
+             * its column, since st_fl is a multiple of 8; its ring slot rec_pos is group aligned.  Lanes read
+             * each other's staging here: the __syncwarp()s order the owners' earlier staging writes before
+             * these reads, and these reads before the owners' next staging writes. */
+            const bool full = (st_wr - st_fl) >= HS_FLUSH;
+            __syncwarp();
+            uint32_t owners = __ballot_sync(0xffffffffu, full);
+            if (owners) {
+                /* everything below is derived from the lane index read here, so none of it is hoisted out
+                 * of the event loop, where registers are scarce; the owner's ring is found from the kernel
+                 * parameters, so only two 32-bit values cross lanes */
+                uint32_t lane;
+                asm volatile("mov.u32 %0, %%laneid;" : "=r"(lane));
+                const uint32_t k = lane & 3u, row = lane >> 2;
+                const uint32_t warp_r0 = blockIdx.x * HS_LANE_THREADS + tid - lane;   /* replica of lane 0 */
+                do {
+                    /* the k-th lowest owner left (32: none); __fns instead of a search loop keeps <10> free of
+                     * spills */
+                    const uint32_t owner = min(__fns(owners, 0u, (int)k + 1), 32u);
+                    uint32_t rest = owners;
+#pragma unroll
+                    for (uint32_t q = 0; q < 4; ++q) rest &= rest - 1u;
+                    const uint32_t src = owner < 32u ? owner : lane;
+                    const uint32_t o_pos = __shfl_sync(0xffffffffu, rec_pos, src);
+                    const uint32_t o_row = __shfl_sync(0xffffffffu, st_fl, src) % HS_STAGE + row;
+                    if (owner < 32u)
+                        __stcs((uint4 *)(O.records + (size_t)(warp_r0 + owner) * P.record_cap + o_pos + row),
+                               sh_rec[o_row][tid - lane + owner]);
+                    owners = rest;
+                } while (owners);
+                __syncwarp();
+                if (full) { st_fl += HS_FLUSH; rec_pos = (rec_pos + HS_FLUSH == P.record_cap) ? 0u : rec_pos + HS_FLUSH; }
+            }
+        }
+        /* SIMPLE: the three shared-memory operands of the next chain, requested before any of them is used:
+         * next arrival time, next service time, queue head */
         int64_t tT_next = 0; double sv_next = 0.0; hs_ring_entry h; h.created = 0; h.idx = 0;
         if (SIMPLE) {
             tT_next = sh_t[(arr_draws + 1) % HS_DRAW_BUF][tid];
             sv_next = sh_svc[(uint32_t)((uint64_t)n_svc % HS_DRAW_BUF)][tid];
             asm volatile("cp.async.wait_group 0;" ::: "memory");
             h = *my_head;                                    /* next queued request (meaningful if q_len > 0) */
-        }
-        if (FLAGS & HS_LF_REC) {
-            /* a lane holding a full 128-byte group writes it itself: 8 reads of its own staging column,
-             * four 256-bit stores (st_fl is a multiple of 8, so the group is rows 0-7 or 8-15) */
-            if (staged && (st_wr - st_fl) >= HS_FLUSH) {
-                const uint4 *src = &sh_rec[st_fl & (HS_STAGE - 1)][tid];
-                uint4 *dst = (uint4 *)(rec + rec_pos);
-#pragma unroll
-                for (int g = 0; g < HS_FLUSH; g += 2)
-                    hs_st256(dst + g, src[(size_t)g * HS_LANE_THREADS], src[(size_t)(g + 1) * HS_LANE_THREADS]);
-                st_fl += HS_FLUSH; rec_pos = (rec_pos + HS_FLUSH == P.record_cap) ? 0u : rec_pos + HS_FLUSH;
-            }
         }
         if (finished) continue;
 
@@ -607,12 +610,13 @@ hs_lane_kernel(hs_lane_model M, hs_lane_run P, hs_lane_state *__restrict__ state
                     }
                     if ((FLAGS & HS_LF_REC) && rec) st_wr += nrec;
                 }
-                /* Two forms of the same updates, chosen per kernel by A/B measurement (tools/bench_lane.py, with
+                /* Two forms of the same updates, chosen by A/B measurement (tools/bench_lane.py, with
                  * HS_LANE_PREDICATED=0/1 builds): selects + predicated memory operations (no branch, no reconvergence
                  * point, no register shuffling where the chains meet again) won without the recorder and with the
-                 * order hash; with the recorder alone the two-branch form won (the predicated Sink block keeps more
-                 * values live across the staged stores). */
-                constexpr bool PREDICATED = HS_LANE_PREDICATED != 0 && (!(FLAGS & HS_LF_REC) || (FLAGS & HS_LF_HASH));
+                 * order hash.  With the recorder alone the two forms run at the same speed (within run-to-run
+                 * spread, profiles/h100_rec_flush_ab.txt), but the two-branch form spills registers next to the
+                 * warp-wide record flush (ptxas: 320 B stack, 64 B spill stores) and the predicated one does not. */
+                constexpr bool PREDICATED = HS_LANE_PREDICATED != 0;
                 if (PREDICATED) {
                 const bool isC = !isA;
                 /* Source: payload index c0, next SourceEvent index c0 + 1 (source.py:166-170) */
