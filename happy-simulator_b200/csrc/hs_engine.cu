@@ -23,9 +23,6 @@
 #include "hs_totals.cuh"
 #include "hs_sketch.h"
 
-struct hs_engine;
-static int hs_warp_launch(hs_engine *E, const hs_run_params *p, uint32_t ring, bool want_hash, bool want_rec, bool want_hist, bool per_thread);
-
 static thread_local char g_err[512] = "";
 
 static int fail(int code, const char *fmt, ...)
@@ -262,12 +259,22 @@ static int validate_model(const hs_model_desc *m)
     return HS_OK;
 }
 
-/* Lane engine eligibility: exactly Source -> Server(c=1) -> Sink|Counter|none. */
+/* a server's concurrency limit, maximised over the sweep cells */
+static int32_t max_concurrency(const hs_engine *E, uint32_t i)
+{
+    const size_t n = E->ents.size();
+    int32_t c = E->ents[i].i0;
+    for (uint32_t k = 0; k < E->n_cells; ++k) c = std::max(c, E->cell_i0[(size_t)k * n + i]);
+    return c;
+}
+
+/* Lane engine eligibility: exactly Source -> Server(concurrency <= 64) -> Sink|Counter|none, and not a partition of a
+ * linked run (the lane kernel has no outbox and no inbox). */
 static bool classify_lane(hs_engine *E)
 {
     const auto &en = E->ents;
     size_t n = en.size();
-    if (n < 2 || n > 3) return false;
+    if (n < 2 || n > 3 || E->outbox_cap || E->inbox_cap) return false;
     int src = -1, srv = -1, dst = -1;
     for (size_t i = 0; i < n; ++i) {
         if (en[i].kind == HS_ENT_SOURCE) { if (src >= 0) return false; src = (int)i; }
@@ -277,10 +284,8 @@ static bool classify_lane(hs_engine *E)
     }
     if (src < 0 || srv < 0) return false;
     if (en[src].target != srv || en[src].i1 != 0) return false;
-    if (en[srv].i0 > 64) return false;
     if (en[srv].target != dst) { if (!(en[srv].target < 0 && dst < 0)) return false; }
-    int32_t c_max = en[srv].i0;
-    for (uint32_t c = 0; c < E->n_cells; ++c) c_max = std::max(c_max, E->cell_i0[(size_t)c * n + srv]);
+    const int32_t c_max = max_concurrency(E, (uint32_t)srv);
     if (c_max > 64) return false;
     hs_lane_model &L = E->lane_model;
     memset(&L, 0, sizeof L);
@@ -300,68 +305,86 @@ static bool classify_lane(hs_engine *E)
 
 static uint32_t pow2_at_least(uint32_t v) { uint32_t p = 1; while (p < v) p <<= 1; return p; }
 
-/* ---- warp / thread engine launch ----------------------------------------- */
+/* ---- one launcher per kernel ----------------------------------------------- */
 
-static int hs_warp_launch(hs_engine *E, const hs_run_params *p, uint32_t ring, bool want_hash, bool want_rec, bool want_hist, bool per_thread)
+/* The launch between the run's two timing events: hs_last_run_ms brackets the kernel alone, so every other piece of
+ * host work (function attributes, uploads, memsets) is issued before this call. */
+template <typename Kernel, typename... Args>
+static int timed_launch(hs_engine *E, Kernel kern, uint32_t blocks, uint32_t threads, size_t smem, Args... args)
 {
-    const uint32_t n = p->n_replicas;
+    CUDA_TRY(cudaEventRecord(E->ev0, E->stream));
+    kern<<<blocks, threads, smem, E->stream>>>(args...);
+    CUDA_TRY(cudaGetLastError());
+    CUDA_TRY(cudaEventRecord(E->ev1, E->stream));
+    E->launches += 1;
+    return HS_OK;
+}
+
+#define HS_K4(K, F) K<F>, K<F + 1>, K<F + 2>, K<F + 3>
+
+static int launch_lane(hs_engine *E, const hs_kernel_run &R, const hs_kernel_out &O, bool want_hash, bool want_rec)
+{
+    const hs_lane_model &M = E->lane_model;
+    const uint32_t n = R.n_replicas;
+    int rc;
+    if ((rc = E->d_state.ensure((size_t)n * sizeof(hs_lane_state)))) return rc;
+    if ((rc = E->d_rings.ensure((size_t)n * R.ring * sizeof(hs_ring_entry)))) return rc;
+    if ((rc = E->d_conts.ensure(std::max<size_t>(64, (size_t)n * M.c_max * sizeof(hs_cont))))) return rc;
+    const bool simple = !M.has_profile && !R.trace_arr && !R.trace_svc && M.arr_kind == HS_ARR_POISSON &&
+                        M.svc_kind == HS_SVC_EXPONENTIAL && M.policy == HS_Q_FIFO && M.capacity < 0 &&
+                        M.stop_after < 0 && M.dst_id >= 0 && M.dst_kind == HS_ENT_SINK && M.c_max == 1;
+    const int fl = (want_hash ? HS_LF_HASH : 0) | (want_rec ? HS_LF_REC : 0) |
+                   (M.has_profile ? HS_LF_PROFILE : 0) | (simple ? HS_LF_SIMPLE : 0);
+    using kernel = void (*)(hs_lane_model, hs_kernel_run, hs_lane_state *, hs_ring_entry *, hs_cont *, hs_kernel_out);
+    static const kernel kernels[] = {HS_K4(hs_lane_kernel, 0), HS_K4(hs_lane_kernel, 4),     /* fl <= 11: the SIMPLE */
+                                     HS_K4(hs_lane_kernel, 8)};                               /* model has no profile */
+    return timed_launch(E, kernels[fl], (n + HS_LANE_THREADS - 1) / HS_LANE_THREADS, HS_LANE_THREADS, 0, M, R,
+                        (hs_lane_state *)E->d_state.p, (hs_ring_entry *)E->d_rings.p, (hs_cont *)E->d_conts.p, O);
+}
+
+static const uint32_t HS_WARP_SMEM_MAX = 227 * 1024 - 1024;      /* dynamic shared memory of a warp-engine CTA */
+
+/* What the warp and the thread engine share: the future-event slots, the servers' queue-ring indices, the replica
+ * state and queue-ring buffers, and the model flags (*fl). */
+static int general_setup(hs_engine *E, const hs_kernel_run &R, bool thread, bool want_hash, bool want_rec,
+                         hs_warp_model &M, int *fl)
+{
+    const uint32_t n = R.n_replicas;
     const uint32_t ne = (uint32_t)E->ents.size();
-    if (!ring) ring = 128;
     /* FEL slots: one pending SourceEvent per source, one ProcessContinuation per busy
      * server slot, plus the same-timestamp protocol events in flight. */
     uint64_t live = 24;
     uint32_t n_servers = 0;
+    bool any_profile = false;
     std::vector<int32_t> srv_index(ne, -1);
     for (uint32_t i = 0; i < ne; ++i) {
         const hs_entity_desc &e = E->ents[i];
-        if (e.kind == HS_ENT_SOURCE) live += 2;
-        if (e.kind == HS_ENT_SERVER) {
-            int32_t c = e.i0;
-            for (uint32_t k = 0; k < E->n_cells; ++k) c = std::max(c, E->cell_i0[(size_t)k * ne + i]);
-            live += (uint64_t)c + 1;
-            srv_index[i] = (int32_t)n_servers++;
-        }
-        if (e.kind == HS_ENT_CACHE_SERVER) {      /* no concurrency limit: one pending continuation per request in service;
-                                                    64 covers 10 000 requests/s through the ~6 ms of a miss (overflow is flagged) */
-            live += 64;
-            srv_index[i] = (int32_t)n_servers++;
-        }
+        if (e.kind == HS_ENT_SOURCE) { live += 2; any_profile = any_profile || e.i3 > 0; }
+        if (e.kind == HS_ENT_SERVER) live += (uint64_t)max_concurrency(E, i) + 1;
+        if (e.kind == HS_ENT_CACHE_SERVER) live += 64;      /* no concurrency limit: one pending continuation per request in service;
+                                                              64 covers 10 000 requests/s through the ~6 ms of a miss (overflow is flagged) */
+        if (e.kind == HS_ENT_SERVER || e.kind == HS_ENT_CACHE_SERVER) srv_index[i] = (int32_t)n_servers++;
     }
     live += E->inbox_cap;                            /* what a barrier can deliver is scheduled at once */
     const uint32_t S = (uint32_t)((live + 31) / 32) * 32;
     if (S > 65535) return fail(HS_ERR_INVALID, "model needs %u future-event slots (limit 65535)", S);
     /* thread engine: 4-ary key heap + payload slots instead of the warp engine's SoA slot table */
-    const uint32_t block_bytes = per_thread
+    const uint32_t block_bytes = thread
         ? hs_thread_offsets(ne, S).total
         : (uint32_t)(sizeof(hs_warp_hdr) + (size_t)ne * sizeof(hs_went) + (((size_t)S * 46 + 15) / 16) * 16 +
                      (size_t)HS_W_NCAP * sizeof(hs_wnow));
-    const uint32_t per_warp = 16 + block_bytes;
-    uint32_t model_bytes = (uint32_t)((ne * sizeof(hs_entity_desc) + ne * 4 + E->backends.size() * 4 + 15) / 16 * 16);
-    if (per_warp + model_bytes > 227 * 1024 - 1024) model_bytes = 0;      /* tables stay in global memory */
-    const uint32_t smem_budget = 200 * 1024;
-    if (!per_thread && per_warp + model_bytes > 227 * 1024 - 1024) return fail(HS_ERR_INVALID, "model too large for the warp engine (%u B of state per replica)", per_warp);
-    uint32_t warps = std::min<uint32_t>(8, std::max<uint32_t>(1, (smem_budget / 2) / per_warp));
-    while (warps > 1 && per_warp * warps + model_bytes > 227 * 1024 - 1024) warps--;
-    const uint32_t smem = per_warp * warps + model_bytes;
-    uint32_t blocks_per_sm = std::max<uint32_t>(1, std::min<uint32_t>((227 * 1024) / (smem + 1024), 64 / warps));
-    if (blocks_per_sm * warps * 32 > 2048) blocks_per_sm = 2048 / (warps * 32);
-    uint32_t grid = std::min<uint32_t>((n + warps - 1) / warps, (uint32_t)E->sm_count * blocks_per_sm);
-
-    if (p->resume && (E->last_ring != ring)) return fail(HS_ERR_STATE, "resume must keep queue_ring");
-    E->last_ring = ring;
+    /* the warp engine stages a replica's block (and an mbarrier slot) in shared memory */
+    if (!thread && 16 + block_bytes > HS_WARP_SMEM_MAX)
+        return fail(HS_ERR_INVALID, "model too large for the warp engine (%u B of state per replica)", 16 + block_bytes);
     int rc;
     if ((rc = E->d_state.ensure((size_t)n * block_bytes))) return rc;
-    if ((rc = E->d_rings.ensure(std::max<size_t>(16, (size_t)n * n_servers * ring * sizeof(hs_wring_entry))))) return rc;
+    if ((rc = E->d_rings.ensure(std::max<size_t>(16, (size_t)n * n_servers * R.ring * sizeof(hs_wring_entry))))) return rc;
     if ((rc = E->d_srv_index.ensure(ne * 4 + 16))) return rc;
-    if ((rc = E->d_counter.ensure(16))) return rc;
     if (E->srv_index_host != srv_index) {            /* uploaded once per model: the window loop of a linked run stays asynchronous */
         E->srv_index_host = srv_index;
         CUDA_TRY(cudaMemcpyAsync(E->d_srv_index.p, E->srv_index_host.data(), ne * 4, cudaMemcpyHostToDevice, E->stream));
         CUDA_TRY(cudaStreamSynchronize(E->stream));
     }
-    CUDA_TRY(cudaMemsetAsync(E->d_counter.p, 0, 16, E->stream));
-
-    hs_warp_model M;
     M.ents = (const hs_entity_desc *)E->d_ents.p;
     M.backends = (const int32_t *)E->d_backends.p; M.key_table = (const int32_t *)E->d_key_table.p;
     M.srv_index = (const int32_t *)E->d_srv_index.p;
@@ -370,128 +393,83 @@ static int hs_warp_launch(hs_engine *E, const hs_run_params *p, uint32_t ring, b
     M.sketch_tables = (const int32_t *)E->d_sketch_tab.p; M.sk_total = E->sk_total;
     M.key_cdf = (const double *)E->d_key_cdf.p;
     M.n_entities = ne; M.n_cells = E->n_cells; M.n_servers = n_servers; M.fel_slots = S; M.block_bytes = block_bytes;
-    {
-        bool fixed = per_thread && ne <= S && E->inbox_cap == 0;      /* delivered events need slots of their own */
-        for (uint32_t i = 0; i < ne && fixed; ++i) {
-            const hs_entity_desc &e = E->ents[i];
-            if (e.kind == HS_ENT_CACHE_SERVER) fixed = false;
-            if (e.kind == HS_ENT_SERVER) {
-                int32_t c = e.i0;
-                for (uint32_t k = 0; k < E->n_cells; ++k) c = std::max(c, E->cell_i0[(size_t)k * ne + i]);
-                if (c != 1) fixed = false;
-            }
-        }
-        M.fixed_slots = fixed ? 1u : 0u; M.pad_ = 0;
-        M.outbox_cap = E->outbox_cap; M.inbox_cap = E->inbox_cap;
-    }
-    M.n_backends = (uint32_t)E->backends.size(); M.model_bytes = model_bytes;
-    hs_warp_run R;
-    R.seed = p->seed; R.seed_stride = p->seed_stride; R.rid_base = p->rid_base; R.rid_stride = p->rid_stride;
-    R.end_ns = p->end_ns; R.window_end_ns = p->window_end_ns;
-    R.n_replicas = n; R.index_base = p->replica_index_base; R.replicas_per_cell = p->replicas_per_cell;
-    R.record_cap = p->record_cap; R.sample_cap = p->sample_cap; R.service_cap = p->service_cap;
-    R.ring = ring; R.resume = p->resume; R.lane_stride = 1; R.heap_top = 0;
-    R.linked = (p->flags & HS_RUN_LINKED) ? 1u : 0u;
-    R.max_events = p->max_events > 0 ? p->max_events : INT64_MAX;
-    R.trace_arr = E->n_trace_arr ? (const double *)E->d_trace_arr.p : nullptr; R.n_trace_arr = E->n_trace_arr;
-    R.trace_svc = E->n_trace_svc ? (const double *)E->d_trace_svc.p : nullptr; R.n_trace_svc = E->n_trace_svc;
-    hs_warp_out O;
-    O.summaries = (hs_replica_summary *)E->d_summ.p; O.stats = (hs_entity_stats *)E->d_stats.p;
-    O.records = p->record_cap ? (hs_event_record *)E->d_rec.p : nullptr;
-    O.samples = p->sample_cap ? (hs_sink_sample *)E->d_smp.p : nullptr;
-    O.service = p->service_cap ? (double *)E->d_svc.p : nullptr;
-    O.hist = want_hist ? (uint32_t *)E->d_hist.p : nullptr;
-    O.sketch = (uint8_t *)E->d_sketch.p;
-    O.outbox = (hs_xevent *)E->d_outbox.p; O.outbox_n = (uint32_t *)E->d_outbox_n.p;
-    O.inbox = (hs_xevent *)E->d_inbox.p; O.inbox_n = (uint32_t *)E->d_inbox_n.p;
-    if ((E->outbox_cap || E->inbox_cap || R.linked) && !per_thread)
-        return fail(HS_ERR_INVALID, "linked partitions run on the thread engine (engine 3)");
-
-    auto launch = [&](auto kern) -> int {
-        CUDA_TRY(cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
-        CUDA_TRY(cudaEventRecord(E->ev0, E->stream));
-        kern<<<grid, warps * 32, smem, E->stream>>>(M, R, (unsigned char *)E->d_state.p, (hs_wring_entry *)E->d_rings.p, O,
-                                                   (unsigned int *)E->d_counter.p);
-        CUDA_TRY(cudaGetLastError());
-        CUDA_TRY(cudaEventRecord(E->ev1, E->stream));
-        return 0;
-    };
-    bool any_profile = false;
-    for (const hs_entity_desc &e : E->ents) if (e.kind == HS_ENT_SOURCE && e.i3 > 0) any_profile = true;
-    const int fl = (want_hash ? HS_WF_HASH : 0) | (want_rec ? HS_WF_REC : 0) | (any_profile ? HS_WF_PROFILE : 0);
-    if (per_thread) {
-        M.model_bytes = 0;
-        /* replicas per warp: enough warps to fill the register file (16 warps of 128 registers per SM),
-         * and no more lanes per warp than that needs -- a warp's iteration costs the sum of the distinct
-         * paths its lanes take.  HS_THREAD_RPW overrides (experiments). */
-        uint32_t rpw = pow2_at_least((uint32_t)((n + (uint64_t)E->sm_count * 16 - 1) / ((uint64_t)E->sm_count * 16)));
-        if (const char *ev = getenv("HS_THREAD_RPW")) rpw = pow2_at_least((uint32_t)std::max(1, atoi(ev)));
-        rpw = std::min<uint32_t>(32, std::max<uint32_t>(1, rpw));
-        R.lane_stride = 32 / rpw;
-        const int tblocks = (int)(((uint64_t)n * R.lane_stride + HS_THREAD_BLOCK - 1) / HS_THREAD_BLOCK);
-        /* shared memory of a block: the now tier (HS_T_KS entries x 48 B per replica column) and, next to it, whole top
-         * levels of the key heap: at most three (1 + 4 + 16 keys) and at most 20 KB per block together.  Shared memory is
-         * carved out of the L1 the replicas' state lives in, and deep levels are read at scattered indices (bank
-         * conflicts): on the 64-server farm at 8 replicas per warp, 5 / 21 / 85 keys per replica in shared memory run at
-         * 8.99e9 / 9.25e9 / 8.71e9 events/s (tools/scan_heaptop.py).  HS_THREAD_HEAPTOP overrides (experiments). */
-        const uint32_t rpb = HS_THREAD_BLOCK / R.lane_stride;
-        {
-            const uint32_t budget = std::min<uint32_t>(21u, (20480u / 16u - HS_T_KS * 3u * rpb) / rpb);          /* keys per replica */
-            uint32_t top = 0, level = 1, total = 0;
-            while (total + level <= budget && total + level <= S) { total += level; level *= HS_T_ARITY; top = total; }
-            if (top < 1 + HS_T_ARITY || R.lane_stride == 32) top = 0;       /* one replica per warp: its heap sits in L1 anyway */
-            if (const char *ev = getenv("HS_THREAD_HEAPTOP")) top = (uint32_t)std::max(0, atoi(ev));
-            R.heap_top = top;
-        }
-        const size_t dyn_smem = (size_t)(HS_T_KS * 3u + R.heap_top) * rpb * 16;
-        if (dyn_smem > 48u * 1024u) return fail(HS_ERR_INVALID, "thread engine: %zu bytes of shared memory per block (HS_THREAD_HEAPTOP too large)", dyn_smem);
-        CUDA_TRY(cudaEventRecord(E->ev0, E->stream));
-#define HS_LAUNCH_THREAD(F) case F: hs_thread_kernel<F><<<tblocks, HS_THREAD_BLOCK, dyn_smem, E->stream>>>(M, R, (unsigned char *)E->d_state.p, (hs_wring_entry *)E->d_rings.p, O); break;
-#define HS_LAUNCH_THREAD_WIDE(F) case F: hs_thread_kernel_wide<F><<<tblocks, HS_THREAD_BLOCK, dyn_smem, E->stream>>>(M, R, (unsigned char *)E->d_state.p, (hs_wring_entry *)E->d_rings.p, O); break;
-        const bool linked_model = E->outbox_cap || E->inbox_cap || R.linked;
-        /* small launches (every block resident at 4 blocks per SM, no shared-memory heap top, not linked): the spill-free
-         * instantiation, see hs_thread_kernel_wide; HS_THREAD_WIDE=0/1 overrides (experiments) */
-        bool wide = !R.heap_top && !linked_model && tblocks <= E->sm_count * HS_T_WIDE_BLOCKS;
-        if (const char *ev = getenv("HS_THREAD_WIDE")) wide = atoi(ev) != 0 && !R.heap_top && !linked_model;
-        if (wide) {
-            switch (fl) {
-            HS_LAUNCH_THREAD_WIDE(0) HS_LAUNCH_THREAD_WIDE(1) HS_LAUNCH_THREAD_WIDE(2) HS_LAUNCH_THREAD_WIDE(3)
-            HS_LAUNCH_THREAD_WIDE(4) HS_LAUNCH_THREAD_WIDE(5) HS_LAUNCH_THREAD_WIDE(6) HS_LAUNCH_THREAD_WIDE(7)
-            default: return fail(HS_ERR_STATE, "no wide thread kernel for flags %d", fl);
-            }
-        } else
-        switch (fl | (R.heap_top ? HS_WF_HEAPTOP : 0) | (linked_model ? HS_WF_LINKED : 0)) {
-        HS_LAUNCH_THREAD(0) HS_LAUNCH_THREAD(1) HS_LAUNCH_THREAD(2) HS_LAUNCH_THREAD(3)
-        HS_LAUNCH_THREAD(4) HS_LAUNCH_THREAD(5) HS_LAUNCH_THREAD(6) HS_LAUNCH_THREAD(7)
-        HS_LAUNCH_THREAD(8) HS_LAUNCH_THREAD(9) HS_LAUNCH_THREAD(10) HS_LAUNCH_THREAD(11)
-        HS_LAUNCH_THREAD(12) HS_LAUNCH_THREAD(13) HS_LAUNCH_THREAD(14) HS_LAUNCH_THREAD(15)
-        HS_LAUNCH_THREAD(16) HS_LAUNCH_THREAD(17) HS_LAUNCH_THREAD(18) HS_LAUNCH_THREAD(19)        /* LINKED */
-        HS_LAUNCH_THREAD(20) HS_LAUNCH_THREAD(21) HS_LAUNCH_THREAD(22) HS_LAUNCH_THREAD(23)
-        HS_LAUNCH_THREAD(24) HS_LAUNCH_THREAD(25) HS_LAUNCH_THREAD(26) HS_LAUNCH_THREAD(27)
-        HS_LAUNCH_THREAD(28) HS_LAUNCH_THREAD(29) HS_LAUNCH_THREAD(30) HS_LAUNCH_THREAD(31)
-        default: return fail(HS_ERR_STATE, "no thread kernel for flags %d", fl);
-        }
-#undef HS_LAUNCH_THREAD
-#undef HS_LAUNCH_THREAD_WIDE
-        CUDA_TRY(cudaGetLastError());
-        CUDA_TRY(cudaEventRecord(E->ev1, E->stream));
-        E->launches += 1;
-        return HS_OK;
-    }
-    switch (fl) {
-    case 0: rc = launch(hs_warp_kernel<0>); break;
-    case 1: rc = launch(hs_warp_kernel<1>); break;
-    case 2: rc = launch(hs_warp_kernel<2>); break;
-    case 3: rc = launch(hs_warp_kernel<3>); break;
-    case 4: rc = launch(hs_warp_kernel<4>); break;
-    case 5: rc = launch(hs_warp_kernel<5>); break;
-    case 6: rc = launch(hs_warp_kernel<6>); break;
-    default: rc = launch(hs_warp_kernel<7>); break;
-    }
-    if (rc) return rc;
-    E->launches += 1;
+    M.n_backends = (uint32_t)E->backends.size(); M.model_bytes = 0;
+    M.outbox_cap = E->outbox_cap; M.inbox_cap = E->inbox_cap;
+    M.fixed_slots = 0; M.pad_ = 0;
+    *fl = (want_hash ? HS_WF_HASH : 0) | (want_rec ? HS_WF_REC : 0) | (any_profile ? HS_WF_PROFILE : 0);
     return HS_OK;
 }
+
+static int launch_warp(hs_engine *E, const hs_kernel_run &R, const hs_kernel_out &O, bool want_hash, bool want_rec)
+{
+    hs_warp_model M;
+    int fl, rc;
+    if ((rc = general_setup(E, R, false, want_hash, want_rec, M, &fl))) return rc;
+    /* per warp its replica's block behind an mbarrier slot; per CTA a copy of the model tables when they fit */
+    const uint32_t ne = M.n_entities;
+    const uint32_t per_warp = 16 + M.block_bytes;
+    M.model_bytes = (uint32_t)((ne * sizeof(hs_entity_desc) + ne * 4 + E->backends.size() * 4 + 15) / 16 * 16);
+    if (per_warp + M.model_bytes > HS_WARP_SMEM_MAX) M.model_bytes = 0;      /* tables stay in global memory */
+    const uint32_t smem_budget = 200 * 1024;
+    uint32_t warps = std::min<uint32_t>(8, std::max<uint32_t>(1, (smem_budget / 2) / per_warp));
+    while (warps > 1 && per_warp * warps + M.model_bytes > HS_WARP_SMEM_MAX) warps--;
+    const uint32_t smem = per_warp * warps + M.model_bytes;
+    uint32_t blocks_per_sm = std::max<uint32_t>(1, std::min<uint32_t>((227 * 1024) / (smem + 1024), 64 / warps));
+    if (blocks_per_sm * warps * 32 > 2048) blocks_per_sm = 2048 / (warps * 32);
+    const uint32_t grid = std::min<uint32_t>((R.n_replicas + warps - 1) / warps, (uint32_t)E->sm_count * blocks_per_sm);
+    if ((rc = E->d_counter.ensure(16))) return rc;
+    CUDA_TRY(cudaMemsetAsync(E->d_counter.p, 0, 16, E->stream));
+    using kernel = void (*)(hs_warp_model, hs_kernel_run, unsigned char *, hs_wring_entry *, hs_kernel_out, unsigned int *);
+    static const kernel kernels[] = {HS_K4(hs_warp_kernel, 0), HS_K4(hs_warp_kernel, 4)};
+    CUDA_TRY(cudaFuncSetAttribute(kernels[fl], cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
+    return timed_launch(E, kernels[fl], grid, warps * 32, smem, M, R, (unsigned char *)E->d_state.p,
+                        (hs_wring_entry *)E->d_rings.p, O, (unsigned int *)E->d_counter.p);
+}
+
+static int launch_thread(hs_engine *E, hs_kernel_run R, const hs_kernel_out &O, bool want_hash, bool want_rec, bool linked)
+{
+    hs_warp_model M;
+    int fl, rc;
+    if ((rc = general_setup(E, R, true, want_hash, want_rec, M, &fl))) return rc;
+    const uint32_t n = R.n_replicas, ne = M.n_entities, S = M.fel_slots;
+    /* entity-owned payload slots: every entity has at most one pending future event; delivered events need slots of their own */
+    bool fixed = ne <= S && E->inbox_cap == 0;
+    for (uint32_t i = 0; i < ne && fixed; ++i) {
+        const int32_t kind = E->ents[i].kind;
+        if (kind == HS_ENT_CACHE_SERVER || (kind == HS_ENT_SERVER && max_concurrency(E, i) != 1)) fixed = false;
+    }
+    M.fixed_slots = fixed ? 1u : 0u;
+    /* replicas per warp: enough warps to fill the register file (16 warps of 128 registers per SM),
+     * and no more lanes per warp than that needs -- a warp's iteration costs the sum of the distinct
+     * paths its lanes take. */
+    const uint32_t rpw = std::min<uint32_t>(32, pow2_at_least((uint32_t)((n + (uint64_t)E->sm_count * 16 - 1) / ((uint64_t)E->sm_count * 16))));
+    R.lane_stride = 32 / rpw;
+    const uint32_t tblocks = (uint32_t)(((uint64_t)n * R.lane_stride + HS_THREAD_BLOCK - 1) / HS_THREAD_BLOCK);
+    /* shared memory of a block: the now tier (HS_T_KS entries x 48 B per replica column) and, next to it, whole top
+     * levels of the key heap: at most three (1 + 4 + 16 keys) and at most 20 KB per block together.  Shared memory is
+     * carved out of the L1 the replicas' state lives in, and deep levels are read at scattered indices (bank
+     * conflicts): on the 64-server farm at 8 replicas per warp, 5 / 21 / 85 keys per replica in shared memory ran at
+     * 8.99e9 / 9.25e9 / 8.71e9 events/s. */
+    const uint32_t rpb = HS_THREAD_BLOCK / R.lane_stride;
+    const uint32_t budget = std::min<uint32_t>(21u, (20480u / 16u - HS_T_KS * 3u * rpb) / rpb);          /* keys per replica */
+    uint32_t top = 0, level = 1, total = 0;
+    while (total + level <= budget && total + level <= S) { total += level; level *= HS_T_ARITY; top = total; }
+    R.heap_top = (top < 1 + HS_T_ARITY || R.lane_stride == 32) ? 0 : top;  /* one replica per warp: its heap sits in L1 anyway */
+    const size_t dyn_smem = (size_t)(HS_T_KS * 3u + R.heap_top) * rpb * 16;
+    using kernel = void (*)(hs_warp_model, hs_kernel_run, unsigned char *, hs_wring_entry *, hs_kernel_out);
+    static const kernel kernels[] = {HS_K4(hs_thread_kernel, 0), HS_K4(hs_thread_kernel, 4), HS_K4(hs_thread_kernel, 8),
+                                     HS_K4(hs_thread_kernel, 12), HS_K4(hs_thread_kernel, 16), HS_K4(hs_thread_kernel, 20),
+                                     HS_K4(hs_thread_kernel, 24), HS_K4(hs_thread_kernel, 28)};
+    static const kernel wide_kernels[] = {HS_K4(hs_thread_kernel_wide, 0), HS_K4(hs_thread_kernel_wide, 4)};
+    /* small launches (every block resident at 4 blocks per SM, no shared-memory heap top, not linked): the spill-free
+     * instantiation, see hs_thread_kernel_wide */
+    const bool wide = !R.heap_top && !linked && tblocks <= (uint32_t)E->sm_count * HS_T_WIDE_BLOCKS;
+    const kernel kern = wide ? wide_kernels[fl]
+                             : kernels[fl | (R.heap_top ? HS_WF_HEAPTOP : 0) | (linked ? HS_WF_LINKED : 0)];
+    return timed_launch(E, kern, tblocks, HS_THREAD_BLOCK, dyn_smem, M, R, (unsigned char *)E->d_state.p,
+                        (hs_wring_entry *)E->d_rings.p, O);
+}
+#undef HS_K4
 
 /* ---- entry points ------------------------------------------------------- */
 
@@ -646,11 +624,15 @@ int hs_run(hs_engine *E, const hs_run_params *p)
 
     if ((E->n_trace_arr || E->n_trace_svc) && p->n_replicas > E->trace_replicas)
         return fail(HS_ERR_INVALID, "hs_set_trace supplied draws for %u replicas, run asks for %u", E->trace_replicas, p->n_replicas);
+    const bool linked = E->outbox_cap || E->inbox_cap || (p->flags & HS_RUN_LINKED);
     int engine = (int)p->engine;
-    if (engine == 0) engine = E->lane_ok ? 2 : 3;
-    if (engine == 2 && !E->lane_ok) return fail(HS_ERR_INVALID, "lane engine needs Source -> Server(concurrency <= 64) -> Sink|Counter");
+    if (engine == 0) engine = E->lane_ok && !linked ? 2 : 3;
     if (engine < 1 || engine > 3) return fail(HS_ERR_INVALID, "unknown engine %d", engine);
+    if (linked && engine != 3) return fail(HS_ERR_INVALID, "linked partitions run on the thread engine (engine 3)");
+    if (engine == 2 && !E->lane_ok) return fail(HS_ERR_INVALID, "lane engine needs Source -> Server(concurrency <= 64) -> Sink|Counter");
 
+    const uint32_t ring = p->queue_ring ? pow2_at_least(p->queue_ring) : engine == 2 ? 256 : 128;
+    const bool want_hist = (p->flags & HS_RUN_HISTOGRAM) != 0;
     if (p->resume) {
         if (!E->have_run) return fail(HS_ERR_STATE, "resume without a previous run");
         const hs_run_params &q = E->last;
@@ -660,11 +642,12 @@ int hs_run(hs_engine *E, const hs_run_params *p)
             q.replica_index_base != p->replica_index_base || q.replicas_per_cell != p->replicas_per_cell ||
             engine != E->last_engine)
             return fail(HS_ERR_STATE, "resume must repeat the replica set, seeds and capacities of the paused run");
+        if (want_hist != E->hist_on) return fail(HS_ERR_STATE, "resume must keep HS_RUN_HISTOGRAM");
+        if (ring != E->last_ring) return fail(HS_ERR_STATE, "resume must keep queue_ring");
     }
 
     const uint32_t n = p->n_replicas;
     const uint32_t ne = (uint32_t)E->ents.size();
-    uint32_t ring = p->queue_ring ? pow2_at_least(p->queue_ring) : 0;
     int rc;
     if ((rc = E->d_summ.ensure((size_t)n * sizeof(hs_replica_summary)))) return rc;
     if ((rc = E->d_stats.ensure((size_t)n * ne * sizeof(hs_entity_stats)))) return rc;
@@ -682,8 +665,6 @@ int hs_run(hs_engine *E, const hs_run_params *p)
         if ((rc = E->d_sketch.ensure((size_t)n * E->sk_total))) return rc;
         if (!p->resume) CUDA_TRY(cudaMemsetAsync(E->d_sketch.p, 0, (size_t)n * E->sk_total, E->stream));
     }
-    const bool want_hist = (p->flags & HS_RUN_HISTOGRAM) != 0;
-    if (p->resume && want_hist != E->hist_on) return fail(HS_ERR_STATE, "resume must keep HS_RUN_HISTOGRAM");
     if (want_hist) {
         if ((rc = E->d_hist.ensure((size_t)n * HS_HISTOGRAM_BINS * sizeof(uint32_t)))) return rc;
         if (!p->resume) CUDA_TRY(cudaMemsetAsync(E->d_hist.p, 0, (size_t)n * HS_HISTOGRAM_BINS * sizeof(uint32_t), E->stream));
@@ -700,61 +681,35 @@ int hs_run(hs_engine *E, const hs_run_params *p)
         }
         E->link_replicas = n;
     }
+
+    hs_kernel_run R;
+    R.seed = p->seed; R.seed_stride = p->seed_stride; R.rid_base = p->rid_base; R.rid_stride = p->rid_stride;
+    R.end_ns = p->end_ns; R.window_end_ns = p->window_end_ns;
+    R.n_replicas = n; R.index_base = p->replica_index_base; R.replicas_per_cell = p->replicas_per_cell;
+    R.record_cap = p->record_cap; R.sample_cap = p->sample_cap; R.service_cap = p->service_cap;
+    R.ring = ring; R.resume = p->resume;
+    R.max_events = p->max_events > 0 ? p->max_events : INT64_MAX;
+    R.trace_arr = E->n_trace_arr ? (const double *)E->d_trace_arr.p : nullptr; R.n_trace_arr = E->n_trace_arr;
+    R.trace_svc = E->n_trace_svc ? (const double *)E->d_trace_svc.p : nullptr; R.n_trace_svc = E->n_trace_svc;
+    R.linked = (p->flags & HS_RUN_LINKED) ? 1u : 0u; R.lane_stride = 1; R.heap_top = 0;
+    hs_kernel_out O;
+    O.summaries = (hs_replica_summary *)E->d_summ.p; O.stats = (hs_entity_stats *)E->d_stats.p;
+    O.records = p->record_cap ? (hs_event_record *)E->d_rec.p : nullptr;
+    O.samples = p->sample_cap ? (hs_sink_sample *)E->d_smp.p : nullptr;
+    O.service = p->service_cap ? (double *)E->d_svc.p : nullptr;
+    O.hist = want_hist ? (uint32_t *)E->d_hist.p : nullptr;
+    O.sketch = (uint8_t *)E->d_sketch.p;
+    O.outbox = (hs_xevent *)E->d_outbox.p; O.outbox_n = (uint32_t *)E->d_outbox_n.p;
+    O.inbox = (hs_xevent *)E->d_inbox.p; O.inbox_n = (uint32_t *)E->d_inbox_n.p;
     const bool want_hash = (p->flags & HS_RUN_ORDER_HASH) != 0;
     const bool want_rec = (p->record_cap | p->sample_cap | p->service_cap) != 0;
-
-    if (engine == 2) {
-        if (!ring) ring = 256;
-        if (p->resume && E->last_ring != ring) return fail(HS_ERR_STATE, "resume must keep queue_ring");
-        E->last_ring = ring;
-        if ((rc = E->d_state.ensure((size_t)n * sizeof(hs_lane_state)))) return rc;
-        if ((rc = E->d_rings.ensure((size_t)n * ring * sizeof(hs_ring_entry)))) return rc;
-        hs_lane_model M = E->lane_model;
-        M.cell_d0 = (const double *)E->d_cell_d0.p;
-        M.cell_i0 = (const int32_t *)E->d_cell_i0.p;
-        if ((rc = E->d_conts.ensure(std::max<size_t>(64, (size_t)n * M.c_max * sizeof(hs_cont))))) return rc;
-        hs_lane_run R;
-        R.seed = p->seed; R.seed_stride = p->seed_stride; R.rid_base = p->rid_base; R.rid_stride = p->rid_stride;
-        R.end_ns = p->end_ns; R.window_end_ns = p->window_end_ns;
-        R.n_replicas = n; R.index_base = p->replica_index_base; R.replicas_per_cell = p->replicas_per_cell;
-        R.record_cap = p->record_cap; R.sample_cap = p->sample_cap; R.service_cap = p->service_cap;
-        R.ring = ring; R.resume = p->resume;
-        R.max_events = p->max_events > 0 ? p->max_events : INT64_MAX;
-        R.trace_arr = E->n_trace_arr ? (const double *)E->d_trace_arr.p : nullptr; R.n_trace_arr = E->n_trace_arr;
-        R.trace_svc = E->n_trace_svc ? (const double *)E->d_trace_svc.p : nullptr; R.n_trace_svc = E->n_trace_svc;
-        hs_lane_out O;
-        O.summaries = (hs_replica_summary *)E->d_summ.p; O.stats = (hs_entity_stats *)E->d_stats.p;
-        O.records = p->record_cap ? (hs_event_record *)E->d_rec.p : nullptr;
-        O.samples = p->sample_cap ? (hs_sink_sample *)E->d_smp.p : nullptr;
-        O.service = p->service_cap ? (double *)E->d_svc.p : nullptr;
-        O.hist = want_hist ? (uint32_t *)E->d_hist.p : nullptr;
-        const int threads = HS_LANE_THREADS;
-        const int blocks = (int)((n + threads - 1) / threads);
-        CUDA_TRY(cudaEventRecord(E->ev0, E->stream));
-        hs_lane_state *st = (hs_lane_state *)E->d_state.p;
-        hs_ring_entry *rg = (hs_ring_entry *)E->d_rings.p;
-        const bool simple = !M.has_profile && !R.trace_arr && !R.trace_svc && M.arr_kind == HS_ARR_POISSON &&
-                            M.svc_kind == HS_SVC_EXPONENTIAL && M.policy == HS_Q_FIFO && M.capacity < 0 &&
-                            M.stop_after < 0 && M.dst_id >= 0 && M.dst_kind == HS_ENT_SINK && M.c_max == 1;
-        const int fl = (want_hash ? HS_LF_HASH : 0) | (want_rec ? HS_LF_REC : 0) |
-                       (M.has_profile ? HS_LF_PROFILE : 0) | (simple ? HS_LF_SIMPLE : 0);
-#define HS_LAUNCH_LANE(F) case F: hs_lane_kernel<F><<<blocks, threads, 0, E->stream>>>(M, R, st, rg, (hs_cont *)E->d_conts.p, O); break;
-        switch (fl) {
-        HS_LAUNCH_LANE(0) HS_LAUNCH_LANE(1) HS_LAUNCH_LANE(2) HS_LAUNCH_LANE(3)
-        HS_LAUNCH_LANE(4) HS_LAUNCH_LANE(5) HS_LAUNCH_LANE(6) HS_LAUNCH_LANE(7)
-        HS_LAUNCH_LANE(8) HS_LAUNCH_LANE(9) HS_LAUNCH_LANE(10) HS_LAUNCH_LANE(11)
-        default: return fail(HS_ERR_STATE, "no lane kernel for flags %d", fl);
-        }
-#undef HS_LAUNCH_LANE
-        CUDA_TRY(cudaGetLastError());
-        CUDA_TRY(cudaEventRecord(E->ev1, E->stream));
-        E->launches += 1;
-    } else {
-        rc = hs_warp_launch(E, p, ring, want_hash, want_rec, want_hist, engine == 3);
-        if (rc) return rc;
-    }
+    rc = engine == 2 ? launch_lane(E, R, O, want_hash, want_rec)
+       : engine == 3 ? launch_thread(E, R, O, want_hash, want_rec, linked)
+       : launch_warp(E, R, O, want_hash, want_rec);
+    if (rc) return rc;
     E->last = *p;
     E->last_engine = engine;
+    E->last_ring = ring;
     E->have_run = true;
     return HS_OK;
 }

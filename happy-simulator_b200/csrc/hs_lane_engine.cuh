@@ -64,7 +64,7 @@
 
 #include "hs_sampler.h"
 #include "hs_profile.h"
-#include "../../include/hs_b200.h"
+#include "hs_kernel_params.cuh"
 
 #define HS_NOW_CAP 8
 #define HS_LANE_THREADS 64
@@ -124,29 +124,6 @@ struct hs_lane_model {
     int32_t has_profile, pad2;        /* 0: ConstantRateProfile fast path         */
 };
 
-struct hs_lane_run {
-    uint64_t seed, seed_stride;
-    uint32_t rid_base, rid_stride;
-    int64_t end_ns, window_end_ns;
-    uint32_t n_replicas, index_base, replicas_per_cell;
-    uint32_t record_cap, sample_cap, service_cap, ring, resume;
-    int64_t max_events;                     /* INT64_MAX = unlimited */
-    const double *trace_arr, *trace_svc;    /* externally supplied draws (hs_set_trace) or NULL */
-    uint64_t n_trace_arr, n_trace_svc;
-};
-
-struct hs_lane_out {
-    hs_replica_summary *summaries;
-    hs_entity_stats *stats;
-    hs_event_record *records;
-    hs_sink_sample *samples;
-    double *service;
-    uint32_t *hist;                   /* [replica][HS_HIST_BINS] or NULL */
-};
-
-#ifndef HS_LANE_PREDICATED
-#define HS_LANE_PREDICATED 1    /* SIMPLE chains: state updates as selects + predicated memory operations (0: two branches) */
-#endif
 /* one full 32-byte sector per lane, as two back-to-back streaming 128-bit stores (STG.E.128, the widest
  * global store of sm_90a): the recorder streams are write-once per ring pass */
 __device__ __forceinline__ void hs_st256(void *p, const uint4 a, const uint4 b)
@@ -172,8 +149,8 @@ __device__ __forceinline__ int64_t hs_lane_next_arrival(int64_t t, double target
 
 template <int FLAGS>
 __global__ void __launch_bounds__(HS_LANE_THREADS, 7)
-hs_lane_kernel(hs_lane_model M, hs_lane_run P, hs_lane_state *__restrict__ states,
-               hs_ring_entry *__restrict__ rings, hs_cont *__restrict__ conts, hs_lane_out O)
+hs_lane_kernel(hs_lane_model M, hs_kernel_run P, hs_lane_state *__restrict__ states,
+               hs_ring_entry *__restrict__ rings, hs_cont *__restrict__ conts, hs_kernel_out O)
 {
     constexpr uint32_t HS_DRAW_BUF = (FLAGS & HS_LF_REC) ? HS_DRAW_BUF_RECORD : HS_DRAW_BUF_SUMMARY;
     constexpr uint32_t STAGE_ROWS = (FLAGS & HS_LF_REC) ? HS_STAGE : 1;
@@ -610,14 +587,12 @@ hs_lane_kernel(hs_lane_model M, hs_lane_run P, hs_lane_state *__restrict__ state
                     }
                     if ((FLAGS & HS_LF_REC) && rec) st_wr += nrec;
                 }
-                /* Two forms of the same updates, chosen by A/B measurement (tools/bench_lane.py, with
-                 * HS_LANE_PREDICATED=0/1 builds): selects + predicated memory operations (no branch, no reconvergence
-                 * point, no register shuffling where the chains meet again) won without the recorder and with the
-                 * order hash.  With the recorder alone the two forms run at the same speed (within run-to-run
-                 * spread, profiles/h100_rec_flush_ab.txt), but the two-branch form spills registers next to the
-                 * warp-wide record flush (ptxas: 320 B stack, 64 B spill stores) and the predicated one does not. */
-                constexpr bool PREDICATED = HS_LANE_PREDICATED != 0;
-                if (PREDICATED) {
+                /* The updates as selects + predicated memory operations, not as one branch per chain: no branch, no
+                 * reconvergence point, no register shuffling where the chains meet again.  Measured A/B against the
+                 * two-branch form (tools/bench_lane.py), it won without the recorder and with the order hash.  With
+                 * the recorder alone the two forms run at the same speed (within run-to-run spread,
+                 * profiles/h100_rec_flush_ab.txt), but the two-branch form spills registers next to the warp-wide
+                 * record flush (ptxas: 320 B stack, 64 B spill stores) and the predicated one does not. */
                 const bool isC = !isA;
                 /* Source: payload index c0, next SourceEvent index c0 + 1 (source.py:166-170) */
                 arr_draws += isA ? 1ull : 0ull;
@@ -671,40 +646,6 @@ hs_lane_kernel(hs_lane_model M, hs_lane_run P, hs_lane_state *__restrict__ state
                 c_created = start ? start_created : c_created;
                 svc_s = start ? sv_next : svc_s;
                 active = start ? 1 : (isA ? active : 0);
-                } else {
-                if (isA) {
-                    /* Source: payload index c0, next SourceEvent index c0 + 1 (source.py:166-170) */
-                    arr_draws++; tT = tT_next; iT = c0 + 1;
-                    if (!start) {                                   /* Queue._handle_enqueue: the request waits */
-                        hs_ring_entry e_; e_.created = now; e_.idx = c0;
-                        ring[(q_head + q_len) & ring_mask] = e_;
-                        if (q_empty) *my_head = e_;
-                        q_len++;
-                    }
-                } else {
-                    /* Server resumes after its yield, the Sink takes the request (server.py:255-273, common.py:36-44) */
-                    total_service = HS_ADD(total_service, svc_s);
-                    HS_SINK(c_created);
-                    active = 0;
-                    if (start) {                                    /* Queue._handle_poll: pop the head, prefetch the next */
-                        q_head++; q_len--;
-                        if (q_len == 0) q_head = 0;                 /* an empty queue restarts at slot 0 (hot lines stay in L2) */
-                        if (q_len > 0) {
-                            const hs_ring_entry *n_ = ring + (q_head & ring_mask);
-                            asm volatile("cp.async.ca.shared.global [%0], [%1], 16;\n\tcp.async.commit_group;"
-                                         :: "r"(my_head_s), "l"(n_) : "memory");
-                        }
-                    }
-                }
-                if (start) {
-                    /* Server.handle_queued_event up to its yield (server.py:217-253): the scheduled
-                     * ProcessContinuation takes the last index of the chain */
-                    const double sv_ = sv_next;
-                    if ((FLAGS & HS_LF_REC) && svc_out) HS_SVC_STORE(sv_);
-                    n_svc++;
-                    tC = now + hs_seconds_to_ns(sv_); iC = ctr - 1; c_created = start_created; svc_s = sv_; active = 1;
-                }
-                }
                 continue;
             }
         }

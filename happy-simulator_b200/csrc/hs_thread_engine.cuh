@@ -36,7 +36,7 @@
 #ifndef HS_THREAD_ENGINE_CUH
 #define HS_THREAD_ENGINE_CUH
 
-#include "hs_warp_engine.cuh"       /* hs_warp_hdr, hs_went, hs_wnow, hs_wring_entry, model/run/out structs */
+#include "hs_warp_engine.cuh"       /* hs_warp_hdr, hs_went and its init / publish, hs_wnow, hs_wring_entry, hs_warp_model */
 
 #define HS_THREAD_BLOCK 64
 #define HS_T_KS 4                   /* now-tier entries per replica held in shared memory */
@@ -75,22 +75,13 @@ __host__ __device__ inline hs_thread_layout hs_thread_offsets(uint32_t ne, uint3
 
 #define HS_T_LT(T1, I1, T2, I2) ((T1) < (T2) || ((T1) == (T2) && (I1) < (I2)))
 
-/* experiment switches (HS_B200_DEFS="-DHS_T_...=0" builds the A/B variants; the defaults are the measured winners) */
-#ifndef HS_T_PREFETCH
-#define HS_T_PREFETCH 1             /* the next chain's payload / entity lines are requested while the current chain runs */
-#endif
-
-#ifndef HS_T_TAILINS
-#define HS_T_TAILINS 1              /* fused chains: heap insertions in ONE place, after tick and completion lanes reconverged */
-#endif
-
 __device__ __forceinline__ void hs_prefetch(const void *p) { asm volatile("prefetch.global.L1 [%0];" :: "l"(p)); }
 
 
 template <int FLAGS>
 __device__ __forceinline__ void
-hs_thread_body(const hs_warp_model &M, const hs_warp_run &P, unsigned char *__restrict__ blocks,
-               hs_wring_entry *__restrict__ rings, const hs_warp_out &O)
+hs_thread_body(const hs_warp_model &M, const hs_kernel_run &P, unsigned char *__restrict__ blocks,
+               hs_wring_entry *__restrict__ rings, const hs_kernel_out &O)
 {
     /* dynamic shared memory of a block: [ now tier: HS_T_KS x 3 chunks x rpb columns | heap top: P.heap_top keys x rpb columns ],
      * rpb = replicas (columns) of the block.  The now tier is sized by the columns in use (it was 64 wide whatever the
@@ -194,18 +185,7 @@ hs_thread_body(const hs_warp_model &M, const hs_warp_run &P, unsigned char *__re
         for (uint32_t i = 0; i < S; ++i) FREE[i] = (uint16_t)(S - 1 - i);
         memset(&hdr, 0, sizeof hdr);
         const uint32_t cell = M.n_cells ? (gidx / P.replicas_per_cell) % M.n_cells : 0u;
-        for (uint32_t i = 0; i < ne; ++i) {
-            const hs_entity_desc d = ENTS[i];
-            hs_went *e = &E[i].w;
-            e->d0 = M.n_cells ? M.cell_d0[(size_t)cell * ne + i] : d.d0;
-            e->i0 = M.n_cells ? M.cell_i0[(size_t)cell * ne + i] : d.i0;
-            if (d.kind == HS_ENT_CACHE_SERVER) e->i0 = 0x7fffffff;          /* Entity.has_capacity() is True: no limit */
-            e->lambda = (d.kind == HS_ENT_SERVER && d.i2 == HS_SVC_EXPONENTIAL) ? HS_DIV(1.0, e->d0) : 0.0;
-            if (d.kind == HS_ENT_SINK || d.kind == HS_ENT_PROBE) {
-                e->u.snk.mn = __longlong_as_double(0x7ff0000000000000LL);
-                e->u.snk.mx = __longlong_as_double(0xfff0000000000000LL);
-            }
-        }
+        for (uint32_t i = 0; i < ne; ++i) hs_went_init(&E[i].w, ENTS[i], M, cell, i);
         h_hash = HS_HASH_INIT;
         /* Simulation.__init__: source.start() in order; bootstrap indices come from the global
          * counter (simulation.py:77,145-154), run() restarts the per-heap one at 0. */
@@ -344,7 +324,6 @@ hs_thread_body(const hs_warp_model &M, const hs_warp_run &P, unsigned char *__re
     hs_tkey pk0, pk1; pk0.time = pk1.time = 0; pk0.k2 = pk1.k2 = 0ull;
     int n_pk = 0;
     auto chain_insert = [&](hs_tkey fkey, const hs_tpay &fpay) {
-        if (!HS_T_TAILINS) { heap_insert(fkey, fpay); return; }
         if (!heap_slot_store(fkey, fpay, (uint32_t)n_pk)) return;
         if (n_pk == 0) pk0 = fkey; else pk1 = fkey;
         n_pk++;
@@ -448,7 +427,7 @@ hs_thread_body(const hs_warp_model &M, const hs_warp_run &P, unsigned char *__re
                 if (resume_t <= now) return false;                   /* a zero-length service resumes at this very nanosecond */
             }
             /* ---- nothing can stop the chain any more: run it ---------------------------------------------------- */
-            if (HS_T_PREFETCH && use_rr) {
+            if (use_rr) {
                 /* round robin: the backend of the NEXT request is the next slot, so its state -- the one load of the next
                  * tick chain that depends on another load -- is requested now.  (A key-table balancer's next backend is
                  * known too, the routing key being a pure function of its draw index, but the extra Philox evaluation
@@ -521,7 +500,7 @@ hs_thread_body(const hs_warp_model &M, const hs_warp_run &P, unsigned char *__re
             int tkind = 0;
             if (tgt >= 0) { tkind = ENTS[tgt].kind; if (tkind != HS_ENT_SINK && tkind != HS_ENT_COUNTER) return false; }
             went_u xv; went_load((int)ent, xv); hs_went *Xv = &xv.w;
-            if (HS_T_PREFETCH && tgt >= 0) hs_prefetch(&E[tgt]);     /* the sink's line: wanted after the draw */
+            if (tgt >= 0) hs_prefetch(&E[tgt]);     /* the sink's line: wanted after the draw */
             const uint32_t q_head = Xv->u.srv.q_head, q_len = Xv->u.srv.q_len;
             const int32_t active = Xv->u.srv.active > 0 ? Xv->u.srv.active - 1 : 0;
             const bool poll = (ev.hook & 0x80000000u) && active < Xv->i0;
@@ -732,12 +711,10 @@ hs_thread_body(const hs_warp_model &M, const hs_warp_run &P, unsigned char *__re
                 }
                 kstore(k, last);
                 if (k == 0) { top_t = last.time; top_k = last.k2; }
-                if (HS_T_PREFETCH) {
-                    /* the new root is (unless this chain schedules something sooner) the NEXT pop: its payload and, with
-                     * entity-owned slots, its entity's state are requested now, a whole chain ahead of their use */
-                    const uint32_t ns = (uint32_t)(top_k & 0xffffu);
-                    hs_prefetch(M.fixed_slots ? (const void *)&E[ns] : (const void *)&PAY[ns]);   /* entity-owned slot: ONE line holds both */
-                }
+                /* the new root is (unless this chain schedules something sooner) the NEXT pop: its payload and, with
+                 * entity-owned slots, its entity's state are requested now, a whole chain ahead of their use */
+                const uint32_t ns = (uint32_t)(top_k & 0xffffu);
+                hs_prefetch(M.fixed_slots ? (const void *)&E[ns] : (const void *)&PAY[ns]);   /* entity-owned slot: ONE line holds both */
             }
             if (heap_n == 0) { top_t = HS_W_EMPTY; top_k = ~0ull; }
             h_fel--;
@@ -755,11 +732,9 @@ hs_thread_body(const hs_warp_model &M, const hs_warp_run &P, unsigned char *__re
                    ev_kind = k; }
             asm volatile("" : "+r"(chain_done), "+r"(n_pk));   /* ONE copy of what follows for the tick and the completion lanes, after
                                                                  * they have reconverged (the compiler would otherwise thread it into both chains) */
-            if (HS_T_TAILINS) {
 #pragma unroll 1
-                for (int i = 0; i < n_pk; ++i) heap_push_key(i == 0 ? pk0 : pk1);
-                n_pk = 0;
-            }
+            for (int i = 0; i < n_pk; ++i) heap_push_key(i == 0 ? pk0 : pk1);
+            n_pk = 0;
             if (chain_done) next_event();
         }
         /* ---- handler phases, in chain order: ONE copy of the handlers (a copy per kind was three times slower when a
@@ -799,28 +774,8 @@ hs_thread_body(const hs_warp_model &M, const hs_warp_run &P, unsigned char *__re
         s.heap_left = h_fel; s.status = hdr.status;
         O.summaries[r] = s;
     }
-    if (O.stats) {
-        for (uint32_t i = 0; i < ne; ++i) {
-            const hs_went *e = &E[i].w;
-            hs_entity_stats a; a.c0 = a.c1 = a.c2 = a.c3 = 0; a.f0 = a.f1 = a.f2 = a.f3 = 0.0;
-            switch (ENTS[i].kind) {
-            case HS_ENT_SOURCE: a.c0 = e->u.src.generated; a.c1 = e->u.src.provider; break;
-            case HS_ENT_SERVER: a.c0 = e->u.srv.accepted; a.c1 = e->u.srv.dropped; a.c2 = e->u.srv.completed;
-                a.c3 = e->u.srv.rejected; a.f0 = e->u.srv.total_service; break;
-            case HS_ENT_CACHE_SERVER: a.c0 = e->u.srv.accepted; a.c1 = e->u.srv.dropped; a.c2 = e->u.srv.completed;
-                a.c3 = e->u.srv.rejected; a.f0 = (double)e->u.srv.svc_draws; a.f1 = (double)e->u.srv.pad; break;   /* misses, hits, size */
-            case HS_ENT_SINK: a.c0 = e->u.snk.received; a.f0 = hs_neumaier_result(e->u.snk.sum, e->u.snk.comp);
-                a.f1 = e->u.snk.sumsq; a.f2 = e->u.snk.mn; a.f3 = e->u.snk.mx; break;
-            case HS_ENT_COUNTER: case HS_ENT_REMOTE: a.c0 = e->u.snk.received; break;
-            case HS_ENT_PROBE: a.c0 = e->u.snk.received; a.f0 = hs_neumaier_result(e->u.snk.sum, e->u.snk.comp);
-                a.f2 = e->u.snk.mn; a.f3 = e->u.snk.mx; break;
-            case HS_ENT_LB: a.c0 = e->u.lb.received; a.c1 = e->u.lb.forwarded; a.c2 = e->u.lb.in_flight;
-                a.c3 = e->u.lb.responses; break;
-            case HS_ENT_SKETCH: a.c0 = e->u.sk.processed; a.c1 = e->u.sk.added; break;
-            }
-            O.stats[(size_t)r * ne + i] = a;
-        }
-    }
+    if (O.stats)
+        for (uint32_t i = 0; i < ne; ++i) O.stats[(size_t)r * ne + i] = hs_went_stats(&E[i].w, ENTS[i].kind);
 }
 
 /* Two entry points around the one body.  hs_thread_kernel: 128 registers per thread, 8 blocks of 64 threads per SM -- the
@@ -831,8 +786,8 @@ hs_thread_body(const hs_warp_model &M, const hs_warp_run &P, unsigned char *__re
  * replicas: 1.125e9 -> 1.25e9 events/s; at 16 384 replicas of configs[2] the wide form would lose a quarter (second wave). */
 template <int FLAGS>
 __global__ void __launch_bounds__(HS_THREAD_BLOCK, HS_T_MINBLOCKS)
-hs_thread_kernel(hs_warp_model M, hs_warp_run P, unsigned char *__restrict__ blocks,
-                 hs_wring_entry *__restrict__ rings, hs_warp_out O)
+hs_thread_kernel(hs_warp_model M, hs_kernel_run P, unsigned char *__restrict__ blocks,
+                 hs_wring_entry *__restrict__ rings, hs_kernel_out O)
 {
     hs_thread_body<FLAGS>(M, P, blocks, rings, O);
 }
@@ -840,8 +795,8 @@ hs_thread_kernel(hs_warp_model M, hs_warp_run P, unsigned char *__restrict__ blo
 #define HS_T_WIDE_BLOCKS 4
 template <int FLAGS>
 __global__ void __launch_bounds__(HS_THREAD_BLOCK, HS_T_WIDE_BLOCKS)
-hs_thread_kernel_wide(hs_warp_model M, hs_warp_run P, unsigned char *__restrict__ blocks,
-                      hs_wring_entry *__restrict__ rings, hs_warp_out O)
+hs_thread_kernel_wide(hs_warp_model M, hs_kernel_run P, unsigned char *__restrict__ blocks,
+                      hs_wring_entry *__restrict__ rings, hs_kernel_out O)
 {
     hs_thread_body<FLAGS>(M, P, blocks, rings, O);
 }

@@ -31,7 +31,7 @@
 #include "hs_sampler.h"
 #include "hs_profile.h"
 #include "hs_sketch.h"
-#include "../../include/hs_b200.h"
+#include "hs_kernel_params.cuh"
 
 #define HS_WF_HASH 1
 #define HS_WF_REC 2
@@ -90,32 +90,43 @@ struct hs_warp_model {
                                          entity id -- no free-slot stack traffic on the heap's push / pop path */
 };
 
-struct hs_warp_run {
-    uint64_t seed, seed_stride;
-    uint32_t rid_base, rid_stride;
-    int64_t end_ns, window_end_ns;
-    uint32_t n_replicas, index_base, replicas_per_cell;
-    uint32_t record_cap, sample_cap, service_cap, ring, resume;
-    uint32_t linked;                /* HS_RUN_LINKED: a window of a linked partition -- finished replicas continue */
-    uint32_t lane_stride;           /* thread engine: lanes per replica (1, 2, 4 ... 32) */
-    uint32_t heap_top;              /* thread engine: number of heap keys (whole top levels: 0, 5, 21, 85 or 341 for
-                                       arity 4) kept in shared memory during a launch, [key][replica column] */
-    int64_t max_events;
-    const double *trace_arr, *trace_svc;
-    uint64_t n_trace_arr, n_trace_svc;
-};
+/* ---- entity rows, shared by the warp and the thread engine ---------------- */
 
-struct hs_warp_out {
-    hs_replica_summary *summaries;
-    hs_entity_stats *stats;
-    hs_event_record *records;
-    hs_sink_sample *samples;
-    double *service;
-    uint32_t *hist;
-    uint8_t *sketch;                /* [replica][sk_total] */
-    hs_xevent *outbox; uint32_t *outbox_n;   /* [replica][outbox_cap], entries used (linked partitions) */
-    hs_xevent *inbox; uint32_t *inbox_n;     /* [replica][inbox_cap], entries waiting to be scheduled   */
-};
+/* a row at the start of a run (the rest of it is zero): the cell's overrides, the CachingServer's unlimited
+ * concurrency, the exponential rate and the Sink / Probe min / max sentinels */
+__device__ __forceinline__ void hs_went_init(hs_went *e, const hs_entity_desc d, const hs_warp_model &M, uint32_t cell, uint32_t i)
+{
+    e->d0 = M.n_cells ? M.cell_d0[(size_t)cell * M.n_entities + i] : d.d0;
+    e->i0 = M.n_cells ? M.cell_i0[(size_t)cell * M.n_entities + i] : d.i0;
+    if (d.kind == HS_ENT_CACHE_SERVER) e->i0 = 0x7fffffff;          /* Entity.has_capacity() is True: no limit */
+    e->lambda = (d.kind == HS_ENT_SERVER && d.i2 == HS_SVC_EXPONENTIAL) ? HS_DIV(1.0, e->d0) : 0.0;
+    if (d.kind == HS_ENT_SINK || d.kind == HS_ENT_PROBE) {
+        e->u.snk.mn = __longlong_as_double(0x7ff0000000000000LL);
+        e->u.snk.mx = __longlong_as_double(0xfff0000000000000LL);
+    }
+}
+
+/* what a row publishes */
+__device__ __forceinline__ hs_entity_stats hs_went_stats(const hs_went *e, int32_t kind)
+{
+    hs_entity_stats a; a.c0 = a.c1 = a.c2 = a.c3 = 0; a.f0 = a.f1 = a.f2 = a.f3 = 0.0;
+    switch (kind) {
+    case HS_ENT_SOURCE: a.c0 = e->u.src.generated; a.c1 = e->u.src.provider; break;
+    case HS_ENT_SERVER: a.c0 = e->u.srv.accepted; a.c1 = e->u.srv.dropped; a.c2 = e->u.srv.completed;
+        a.c3 = e->u.srv.rejected; a.f0 = e->u.srv.total_service; break;
+    case HS_ENT_CACHE_SERVER: a.c0 = e->u.srv.accepted; a.c1 = e->u.srv.dropped; a.c2 = e->u.srv.completed;
+        a.c3 = e->u.srv.rejected; a.f0 = (double)e->u.srv.svc_draws; a.f1 = (double)e->u.srv.pad; break;   /* misses, hits, size */
+    case HS_ENT_SINK: a.c0 = e->u.snk.received; a.f0 = hs_neumaier_result(e->u.snk.sum, e->u.snk.comp);
+        a.f1 = e->u.snk.sumsq; a.f2 = e->u.snk.mn; a.f3 = e->u.snk.mx; break;
+    case HS_ENT_COUNTER: case HS_ENT_REMOTE: a.c0 = e->u.snk.received; break;
+    case HS_ENT_PROBE: a.c0 = e->u.snk.received; a.f0 = hs_neumaier_result(e->u.snk.sum, e->u.snk.comp);
+        a.f2 = e->u.snk.mn; a.f3 = e->u.snk.mx; break;
+    case HS_ENT_LB: a.c0 = e->u.lb.received; a.c1 = e->u.lb.forwarded; a.c2 = e->u.lb.in_flight;
+        a.c3 = e->u.lb.responses; break;
+    case HS_ENT_SKETCH: a.c0 = e->u.sk.processed; a.c1 = e->u.sk.added; break;
+    }
+    return a;
+}
 
 /* ---- PTX helpers: mbarrier + TMA 1-D bulk copies ------------------------- */
 __device__ __forceinline__ uint32_t hs_smem_u32(const void *p) { return (uint32_t)__cvta_generic_to_shared(p); }
@@ -168,8 +179,8 @@ __device__ __forceinline__ void hs_tma_store_1d(void *gmem_dst, const void *smem
 
 template <int FLAGS>
 __global__ void __launch_bounds__(256)
-hs_warp_kernel(hs_warp_model M, hs_warp_run P, unsigned char *__restrict__ blocks,
-               hs_wring_entry *__restrict__ rings, hs_warp_out O, unsigned int *__restrict__ next_replica)
+hs_warp_kernel(hs_warp_model M, hs_kernel_run P, unsigned char *__restrict__ blocks,
+               hs_wring_entry *__restrict__ rings, hs_kernel_out O, unsigned int *__restrict__ next_replica)
 {
     extern __shared__ __align__(16) unsigned char smem_raw[];
     const int lane = threadIdx.x & 31;
@@ -241,18 +252,7 @@ hs_warp_kernel(hs_warp_model M, hs_warp_run P, unsigned char *__restrict__ block
             __syncwarp();
             for (uint32_t i = lane; i < S; i += 32) { f_time[i] = HS_W_EMPTY; f_free[i] = (uint16_t)(S - 1 - i); }
             const uint32_t cell = M.n_cells ? (gidx / P.replicas_per_cell) % M.n_cells : 0u;
-            for (uint32_t i = lane; i < ne; i += 32) {
-                const hs_entity_desc d = ENTS[i];
-                hs_went *e = &E[i];
-                e->d0 = M.n_cells ? M.cell_d0[(size_t)cell * ne + i] : d.d0;
-                e->i0 = M.n_cells ? M.cell_i0[(size_t)cell * ne + i] : d.i0;
-                e->lambda = (d.kind == HS_ENT_SERVER && d.i2 == HS_SVC_EXPONENTIAL) ? HS_DIV(1.0, e->d0) : 0.0;
-                if (d.kind == HS_ENT_CACHE_SERVER) e->i0 = 0x7fffffff;      /* Entity.has_capacity() is True: no limit */
-                if (d.kind == HS_ENT_SINK || d.kind == HS_ENT_PROBE) {
-                    e->u.snk.mn = __longlong_as_double(0x7ff0000000000000LL);
-                    e->u.snk.mx = __longlong_as_double(0xfff0000000000000LL);
-                }
-            }
+            for (uint32_t i = lane; i < ne; i += 32) hs_went_init(&E[i], ENTS[i], M, cell, i);
             __syncwarp();
             if (lane == 0) {
                 H->hash = HS_HASH_INIT;
@@ -420,28 +420,8 @@ hs_warp_kernel(hs_warp_model M, hs_warp_run P, unsigned char *__restrict__ block
             }
         }
         __syncwarp();
-        if (O.stats) {
-            for (uint32_t i = lane; i < ne; i += 32) {
-                const hs_went *e = &E[i];
-                hs_entity_stats a; a.c0 = a.c1 = a.c2 = a.c3 = 0; a.f0 = a.f1 = a.f2 = a.f3 = 0.0;
-                switch (ENTS[i].kind) {
-                case HS_ENT_SOURCE: a.c0 = e->u.src.generated; a.c1 = e->u.src.provider; break;
-                case HS_ENT_SERVER: a.c0 = e->u.srv.accepted; a.c1 = e->u.srv.dropped; a.c2 = e->u.srv.completed;
-                    a.c3 = e->u.srv.rejected; a.f0 = e->u.srv.total_service; break;
-                case HS_ENT_CACHE_SERVER: a.c0 = e->u.srv.accepted; a.c1 = e->u.srv.dropped; a.c2 = e->u.srv.completed;
-                    a.c3 = e->u.srv.rejected; a.f0 = (double)e->u.srv.svc_draws; a.f1 = (double)e->u.srv.pad; break;   /* misses, hits, size */
-                case HS_ENT_SINK: a.c0 = e->u.snk.received; a.f0 = hs_neumaier_result(e->u.snk.sum, e->u.snk.comp);
-                    a.f1 = e->u.snk.sumsq; a.f2 = e->u.snk.mn; a.f3 = e->u.snk.mx; break;
-                case HS_ENT_COUNTER: a.c0 = e->u.snk.received; break;
-                case HS_ENT_PROBE: a.c0 = e->u.snk.received; a.f0 = hs_neumaier_result(e->u.snk.sum, e->u.snk.comp);
-                    a.f2 = e->u.snk.mn; a.f3 = e->u.snk.mx; break;
-                case HS_ENT_LB: a.c0 = e->u.lb.received; a.c1 = e->u.lb.forwarded; a.c2 = e->u.lb.in_flight;
-                    a.c3 = e->u.lb.responses; break;
-                case HS_ENT_SKETCH: a.c0 = e->u.sk.processed; a.c1 = e->u.sk.added; break;
-                }
-                O.stats[(size_t)r * ne + i] = a;
-            }
-        }
+        if (O.stats)
+            for (uint32_t i = lane; i < ne; i += 32) O.stats[(size_t)r * ne + i] = hs_went_stats(&E[i], ENTS[i].kind);
         hs_fence_async_smem();
         __syncwarp();
         if (lane == 0) hs_tma_store_1d(gblk, blk, M.block_bytes);

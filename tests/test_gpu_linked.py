@@ -98,6 +98,18 @@ def test_linked_models_need_the_thread_engine_and_an_outbox():
         m.outbox_cap = 0
         with pytest.raises(engine.EngineError, match="outbox_cap"):
             e.upload(m)
+        # a link destination shaped like the lane engine's model: the lane kernel has no inbox, so the thread engine
+        # runs it -- refused when asked for explicitly, chosen by auto selection (a window of it resumes on engine 3)
+        import happysim_b200 as hs
+        m = hs.mm1()
+        m.inbox_cap = 16
+        e.upload(m)
+        with pytest.raises(engine.EngineError, match="thread engine"):
+            e.run(engine.make_params(seed=1, end_ns=10**10, engine=2))
+        e.run(engine.make_params(seed=1, end_ns=10**10, window_end_ns=5 * 10**9, engine=0))
+        e.run(engine.make_params(seed=1, end_ns=10**10, resume=1, engine=3))
+        s = e.read_outputs()["summaries"]
+        assert int(s["status"][0]) == 0 and int(s["events_processed"][0]) > 0
     finally:
         e.close()
 

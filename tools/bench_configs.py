@@ -6,9 +6,7 @@ sys.path[:0] = [ROOT]
 import happysim_b200 as hs
 from happysim_b200 import engine
 
-def run(name, model, n, end_s, rpw=None, **kw):
-    if rpw is None: os.environ.pop("HS_THREAD_RPW", None)
-    else: os.environ["HS_THREAD_RPW"] = str(rpw); name += f" rpw={rpw}"
+def run(name, model, n, end_s, **kw):
     eng = engine.Engine(0)
     eng.upload(model)
     best = None
@@ -26,14 +24,12 @@ if __name__ == "__main__":
     run("configs[1] mm1 lane engine", hs.mm1(), 65536, 1000.0)
     run("configs[1] mm1 on the WARP engine", hs.mm1(), 65536, 50.0, engine=1)
     run("configs[1] mm1 on the THREAD engine", hs.mm1(), 65536, 50.0, engine=3)
-    for n, rpws in ((4096, (None,)), (16384, (None, 32)), (65536, (None,)), (262144, (None,))):
-        for rpw in rpws:
-            run("configs[2] lb-rr64 thread", hs.lb_round_robin(64, 512.0), n, 10.0, rpw=rpw, engine=3)
+    for n in (4096, 16384, 65536, 262144):
+        run("configs[2] lb-rr64 thread", hs.lb_round_robin(64, 512.0), n, 10.0, engine=3)
     run("configs[2] lb-rr 64 servers, warp", hs.lb_round_robin(64, 512.0), 16384, 10.0, engine=1)
     tab = hs.consistent_hash_table([f"S{i}" for i in range(1024)], 100, 10000)
-    for n, rpws in ((1024, (None,)), (4096, (None,))):
-        for rpw in rpws:
-            run("configs[3] chash1024 thread", hs.lb_key_table(tab, 1024, rate=8192.0), n, 2.0, rpw=rpw, engine=3)
+    for n in (1024, 4096):
+        run("configs[3] chash1024 thread", hs.lb_key_table(tab, 1024, rate=8192.0), n, 2.0, engine=3)
     run("configs[3] chash 1024 nodes, warp", hs.lb_key_table(tab, 1024, rate=8192.0), 1024, 2.0, engine=1)
     K = 10000
     b = hs.ModelBuilder()

@@ -5,9 +5,7 @@ sys.path[:0] = [ROOT]
 import happysim_b200 as hs
 from happysim_b200 import engine
 
-def run(name, model, n, end_s, rpw=None, **kw):
-    if rpw is None: os.environ.pop("HS_THREAD_RPW", None)
-    else: os.environ["HS_THREAD_RPW"] = str(rpw); name += f" rpw={rpw}"
+def run(name, model, n, end_s, **kw):
     eng = engine.Engine(0)
     eng.upload(model)
     best = None
@@ -21,9 +19,8 @@ def run(name, model, n, end_s, rpw=None, **kw):
     eng.close()
 
 lb = hs.lb_round_robin(64, 512.0)
-for n, rpws in ((16384, (None, 16)), (65536, (None, 16, 8))):
-    for rpw in rpws:
-        run("configs[2] lb-rr64", lb, n, 10.0, rpw=rpw)
+for n in (16384, 65536):
+    run("configs[2] lb-rr64", lb, n, 10.0)
 tab = hs.consistent_hash_table([f"S{i}" for i in range(1024)], 100, 10000)
 ch = hs.lb_key_table(tab, 1024, rate=8192.0)
 for n in (1024, 4096):
