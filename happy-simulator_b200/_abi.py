@@ -3,7 +3,7 @@ from __future__ import annotations
 
 import ctypes as C
 
-HS_ABI_VERSION = 4
+HS_ABI_VERSION = 5
 
 HS_OK, HS_ERR_INVALID, HS_ERR_CUDA, HS_ERR_NO_DEVICE, HS_ERR_STATE, HS_ERR_OVERFLOW = 0, -1, -2, -3, -4, -5
 
@@ -110,12 +110,23 @@ class CellTotals(C.Structure):
     _fields_ = [("totals", Totals), ("histogram", C.c_uint64 * 64)]
 
 
+HS_KERNEL_LANE, HS_KERNEL_WARP, HS_KERNEL_THREAD, HS_KERNEL_THREAD_WIDE = 1, 2, 3, 4
+KERNEL_NAMES = {HS_KERNEL_LANE: "lane", HS_KERNEL_WARP: "warp", HS_KERNEL_THREAD: "thread",
+                HS_KERNEL_THREAD_WIDE: "thread_wide"}
+
+
+class LaunchInfo(C.Structure):
+    _fields_ = [("engine", C.c_uint32), ("kernel", C.c_uint32), ("flags", C.c_uint32), ("lane_stride", C.c_uint32),
+                ("heap_top", C.c_uint32), ("grid", C.c_uint32), ("block", C.c_uint32), ("smem", C.c_uint32)]
+
+
 assert C.sizeof(EntityDesc) == 48
 assert C.sizeof(ReplicaSummary) == 56
 assert C.sizeof(EntityStats) == 64
 assert C.sizeof(EventRecord) == 16
 assert C.sizeof(SinkSample) == 16
 assert C.sizeof(RunParams) == 88
+assert C.sizeof(LaunchInfo) == 32
 HS_RUN_ORDER_HASH = 1
 HS_RUN_HISTOGRAM = 2
 HS_HISTOGRAM_BINS = 64

@@ -62,6 +62,7 @@ struct hs_engine {
     bool own_stream = false;
     cudaEvent_t ev0 = nullptr, ev1 = nullptr;
     uint64_t launches = 0;
+    hs_launch_info last_launch = {};                /* engine == 0: nothing launched yet */
     int sm_count = 132;
 
     /* model (host copy + device copy) */
@@ -308,15 +309,17 @@ static uint32_t pow2_at_least(uint32_t v) { uint32_t p = 1; while (p < v) p <<= 
 /* ---- one launcher per kernel ----------------------------------------------- */
 
 /* The launch between the run's two timing events: hs_last_run_ms brackets the kernel alone, so every other piece of
- * host work (function attributes, uploads, memsets) is issued before this call. */
+ * host work (function attributes, uploads, memsets) is issued before this call.  `info` is the launch's geometry
+ * (grid, block, smem) and what hs_last_launch reports of it. */
 template <typename Kernel, typename... Args>
-static int timed_launch(hs_engine *E, Kernel kern, uint32_t blocks, uint32_t threads, size_t smem, Args... args)
+static int timed_launch(hs_engine *E, const hs_launch_info &info, Kernel kern, Args... args)
 {
     CUDA_TRY(cudaEventRecord(E->ev0, E->stream));
-    kern<<<blocks, threads, smem, E->stream>>>(args...);
+    kern<<<info.grid, info.block, info.smem, E->stream>>>(args...);
     CUDA_TRY(cudaGetLastError());
     CUDA_TRY(cudaEventRecord(E->ev1, E->stream));
     E->launches += 1;
+    E->last_launch = info;
     return HS_OK;
 }
 
@@ -338,8 +341,10 @@ static int launch_lane(hs_engine *E, const hs_kernel_run &R, const hs_kernel_out
     using kernel = void (*)(hs_lane_model, hs_kernel_run, hs_lane_state *, hs_ring_entry *, hs_cont *, hs_kernel_out);
     static const kernel kernels[] = {HS_K4(hs_lane_kernel, 0), HS_K4(hs_lane_kernel, 4),     /* fl <= 11: the SIMPLE */
                                      HS_K4(hs_lane_kernel, 8)};                               /* model has no profile */
-    return timed_launch(E, kernels[fl], (n + HS_LANE_THREADS - 1) / HS_LANE_THREADS, HS_LANE_THREADS, 0, M, R,
-                        (hs_lane_state *)E->d_state.p, (hs_ring_entry *)E->d_rings.p, (hs_cont *)E->d_conts.p, O);
+    const hs_launch_info info = {2, HS_KERNEL_LANE, (uint32_t)fl, 1, 0, (n + HS_LANE_THREADS - 1) / HS_LANE_THREADS,
+                                 HS_LANE_THREADS, 0};
+    return timed_launch(E, info, kernels[fl], M, R, (hs_lane_state *)E->d_state.p, (hs_ring_entry *)E->d_rings.p,
+                        (hs_cont *)E->d_conts.p, O);
 }
 
 static const uint32_t HS_WARP_SMEM_MAX = 227 * 1024 - 1024;      /* dynamic shared memory of a warp-engine CTA */
@@ -422,7 +427,8 @@ static int launch_warp(hs_engine *E, const hs_kernel_run &R, const hs_kernel_out
     using kernel = void (*)(hs_warp_model, hs_kernel_run, unsigned char *, hs_wring_entry *, hs_kernel_out, unsigned int *);
     static const kernel kernels[] = {HS_K4(hs_warp_kernel, 0), HS_K4(hs_warp_kernel, 4)};
     CUDA_TRY(cudaFuncSetAttribute(kernels[fl], cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
-    return timed_launch(E, kernels[fl], grid, warps * 32, smem, M, R, (unsigned char *)E->d_state.p,
+    const hs_launch_info info = {1, HS_KERNEL_WARP, (uint32_t)fl, 1, 0, grid, warps * 32, smem};
+    return timed_launch(E, info, kernels[fl], M, R, (unsigned char *)E->d_state.p,
                         (hs_wring_entry *)E->d_rings.p, O, (unsigned int *)E->d_counter.p);
 }
 
@@ -464,9 +470,10 @@ static int launch_thread(hs_engine *E, hs_kernel_run R, const hs_kernel_out &O, 
     /* small launches (every block resident at 4 blocks per SM, no shared-memory heap top, not linked): the spill-free
      * instantiation, see hs_thread_kernel_wide */
     const bool wide = !R.heap_top && !linked && tblocks <= (uint32_t)E->sm_count * HS_T_WIDE_BLOCKS;
-    const kernel kern = wide ? wide_kernels[fl]
-                             : kernels[fl | (R.heap_top ? HS_WF_HEAPTOP : 0) | (linked ? HS_WF_LINKED : 0)];
-    return timed_launch(E, kern, tblocks, HS_THREAD_BLOCK, dyn_smem, M, R, (unsigned char *)E->d_state.p,
+    if (!wide) fl |= (R.heap_top ? HS_WF_HEAPTOP : 0) | (linked ? HS_WF_LINKED : 0);
+    const hs_launch_info info = {3, wide ? (uint32_t)HS_KERNEL_THREAD_WIDE : (uint32_t)HS_KERNEL_THREAD, (uint32_t)fl,
+                                 R.lane_stride, R.heap_top, tblocks, HS_THREAD_BLOCK, (uint32_t)dyn_smem};
+    return timed_launch(E, info, wide ? wide_kernels[fl] : kernels[fl], M, R, (unsigned char *)E->d_state.p,
                         (hs_wring_entry *)E->d_rings.p, O);
 }
 #undef HS_K4
@@ -758,6 +765,14 @@ int hs_launch_count(hs_engine *E, uint64_t *n)
 {
     if (!E || !n) return fail(HS_ERR_INVALID, "NULL argument");
     *n = E->launches;
+    return HS_OK;
+}
+
+int hs_last_launch(hs_engine *E, hs_launch_info *out)
+{
+    if (!E || !out) return fail(HS_ERR_INVALID, "NULL argument");
+    if (!E->last_launch.engine) return fail(HS_ERR_STATE, "no run yet");
+    *out = E->last_launch;
     return HS_OK;
 }
 

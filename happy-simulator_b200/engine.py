@@ -27,7 +27,7 @@ _lib = None
 
 EXPORTED_SYMBOLS = ["hs_version", "hs_last_error", "hs_engine_create", "hs_engine_destroy", "hs_model_upload",
                     "hs_model_validate", "hs_run", "hs_set_trace", "hs_sync", "hs_last_run_ms", "hs_launch_count",
-                    "hs_read_outputs", "hs_read_totals", "hs_read_cell_totals", "hs_totals_device_ptr",
+                    "hs_last_launch", "hs_read_outputs", "hs_read_totals", "hs_read_cell_totals", "hs_totals_device_ptr",
                     "hs_sketch_layout", "hs_read_sketches", "hs_coordinator_create", "hs_coordinator_destroy",
                     "hs_coordinator_exchange", "hs_coordinator_read", "hs_read_outbox", "hs_read_inbox"]
 
@@ -41,6 +41,11 @@ def load_library(path: str | None = None):
     if not os.path.exists(p):
         raise EngineError(A.HS_ERR_STATE, f"{p} not built; run `python -c 'import __graft_entry__ as g; g.build()'`")
     L = C.CDLL(p)
+    # the version first: a library built from older sources says so, instead of lacking a newer entry point below
+    L.hs_version.argtypes, L.hs_version.restype = [], C.c_uint32
+    if L.hs_version() != A.HS_ABI_VERSION:
+        raise EngineError(A.HS_ERR_STATE, f"{p} has ABI version {L.hs_version()}, this package needs {A.HS_ABI_VERSION}; "
+                                          "rebuild it with `python -c 'import __graft_entry__ as g; g.build()'`")
     H = C.c_void_p
     sigs = {
         "hs_version": ([], C.c_uint32),
@@ -54,6 +59,7 @@ def load_library(path: str | None = None):
         "hs_sync": ([H], C.c_int),
         "hs_last_run_ms": ([H, C.POINTER(C.c_float)], C.c_int),
         "hs_launch_count": ([H, C.POINTER(C.c_uint64)], C.c_int),
+        "hs_last_launch": ([H, C.POINTER(A.LaunchInfo)], C.c_int),
         "hs_read_outputs": ([H, C.POINTER(A.Outputs)], C.c_int),
         "hs_read_totals": ([H, C.POINTER(A.Totals)], C.c_int),
         "hs_read_cell_totals": ([H, C.POINTER(A.CellTotals), C.c_uint32], C.c_int),
@@ -205,6 +211,15 @@ class Engine:
         n = C.c_uint64()
         _check(self._L, self._L.hs_launch_count(self._h, C.byref(n)))
         return int(n.value)
+
+    def last_launch(self) -> dict:
+        """The kernel the last run launched and its geometry (hs_last_launch): engine, kernel family ("lane", "warp",
+        "thread", "thread_wide"), template flags, lane_stride, heap_top, grid, block, smem."""
+        li = A.LaunchInfo()
+        _check(self._L, self._L.hs_last_launch(self._h, C.byref(li)))
+        d = {f: int(getattr(li, f)) for f, _ in A.LaunchInfo._fields_}
+        d["kernel"] = A.KERNEL_NAMES[d["kernel"]]
+        return d
 
     def alloc_host_outputs(self, params: A.RunParams | None = None, *, pinned: bool = False):
         """Caller-owned host buffers shaped for ``params`` (numpy; pinned via torch if asked)."""

@@ -28,7 +28,7 @@
 extern "C" {
 #endif
 
-#define HS_ABI_VERSION 4u
+#define HS_ABI_VERSION 5u
 
 typedef enum hs_status {
     HS_OK = 0,
@@ -383,6 +383,20 @@ int hs_last_run_ms(hs_engine *e, float *ms);
 
 /* Number of kernels hs_run launched since engine creation. */
 int hs_launch_count(hs_engine *e, uint64_t *n);
+
+/* Which compiled kernel the last hs_run launched, and its geometry.  The engines pick their kernel from the
+ * model, the ensemble size and the device's SM count; this reports the choice without changing it. */
+enum { HS_KERNEL_LANE = 1, HS_KERNEL_WARP = 2, HS_KERNEL_THREAD = 3, HS_KERNEL_THREAD_WIDE = 4 };
+typedef struct hs_launch_info {
+    uint32_t engine;               /* 1 warp, 2 lane, 3 thread (hs_run_params.engine after auto selection) */
+    uint32_t kernel;               /* HS_KERNEL_* family */
+    uint32_t flags;                /* template FLAGS of the launched instantiation (HS_LF_* / HS_WF_* of csrc/) */
+    uint32_t lane_stride;          /* thread engine: lanes per replica (32 / replicas per warp); 1 otherwise */
+    uint32_t heap_top;             /* thread engine: heap keys per replica held in shared memory; 0 otherwise */
+    uint32_t grid, block;          /* blocks, threads per block */
+    uint32_t smem;                 /* dynamic shared memory per block, bytes */
+} hs_launch_info;      /* 32 bytes */
+int hs_last_launch(hs_engine *e, hs_launch_info *out);
 
 /* Copy results of the last run to caller-owned host buffers (synchronises). */
 int hs_read_outputs(hs_engine *e, const hs_outputs *out);

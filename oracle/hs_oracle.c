@@ -595,8 +595,10 @@ static void orun_until(orun *Rp, int64_t end_ns, int64_t cut_ns)
 #define R (*Rp)
     const hs_run_params *p = R.p;
     while (R.heap.n && R.now <= end_ns) {
-        if (cut_ns >= 0 && R.heap.a[0].time > cut_ns) break;
+        /* the limit before the cut: a replica that has processed max_events has stopped (hs_run_params.max_events),
+         * whether or not its next event lies beyond the window -- as every engine decides it */
         if (p->max_events > 0 && R.processed >= p->max_events) { R.status |= HS_ST_EVENT_LIMIT; break; }
+        if (cut_ns >= 0 && R.heap.a[0].time > cut_ns) break;
         oev e = heap_pop(&R.heap);
         if (e.time < R.now) continue;     /* "time travel": skipped, not counted (simulation.py:479-489) */
         R.now = e.time;

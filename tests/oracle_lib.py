@@ -104,6 +104,46 @@ def oracle_run(model: happysim_b200.FlatModel, p: A.RunParams, r0=None, r1=None)
     return bufs
 
 
+def _pool_map(fn, items):
+    from concurrent.futures import ThreadPoolExecutor
+    lib()                                       # load once, before the threads
+    with ThreadPoolExecutor(max_workers=os.cpu_count() or 1) as ex:
+        return list(ex.map(fn, items))
+
+
+def oracle_run_parallel(model: happysim_b200.FlatModel, p: A.RunParams, chunk: int = 256):
+    """oracle_run on a thread pool: hs_oracle_run_range over slices of ``chunk`` replicas into one set of buffers
+    (ctypes releases the GIL for the call, and a replica only writes its own rows)."""
+    d = model.desc()
+    bufs, o = alloc_outputs(model.n_entities, p, model.sketch_layout()[2])
+    n = p.n_replicas
+
+    def part(r0):
+        assert lib().hs_oracle_run_range(C.byref(d), C.byref(p), C.byref(o), r0, min(n, r0 + chunk)) == 0
+
+    _pool_map(part, range(0, n, chunk))
+    return bufs
+
+
+def oracle_run_linked_parallel(lm, params: list, *, end_ns, cseed, chunk: int = 64):
+    """oracle_run_linked on a thread pool: slices of ``chunk`` replicas (replica_index_base moved along, so every
+    replica keeps its global index and therefore its draws), concatenated in replica order."""
+    n = params[0].n_replicas
+
+    def part(r0):
+        ps = []
+        for p in params:
+            q = A.RunParams.from_buffer_copy(p)
+            q.n_replicas, q.replica_index_base = min(n, r0 + chunk) - r0, p.replica_index_base + r0
+            ps.append(q)
+        return oracle_run_linked(lm, ps, end_ns=end_ns, cseed=cseed)
+
+    parts = _pool_map(part, range(0, n, chunk))
+    outs = [{k: (None if v is None else np.concatenate([pt[0][q][k] for pt in parts])) for k, v in parts[0][0][q].items()}
+            for q in range(lm.n_partitions)]
+    return outs, np.concatenate([pt[1] for pt in parts]), np.concatenate([pt[2] for pt in parts]), parts[0][3]
+
+
 def oracle_run_linked(lm, params: list, *, end_ns, cseed, cseed_stride=0, crid_base=None, crid_stride=None):
     """A linked run (happysim_b200.linked.LinkedModel) on the oracle: per partition the usual output buffers,
     plus per-replica counts of delivered / lost cross-partition events."""

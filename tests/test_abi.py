@@ -40,6 +40,24 @@ def test_version_and_struct_layouts(lib):
     assert C.sizeof(A.EventRecord) == 16 and C.sizeof(A.SinkSample) == 16
     assert C.sizeof(A.LinkDesc) == 24 and A.XEVENT_DTYPE.itemsize == 40          # hs_link_desc, hs_xevent
     assert C.sizeof(A.Totals) == 8 * (A.HS_TOTALS_I64 + A.HS_TOTALS_F64_SUM + 2)
+    assert f"#define HS_ABI_VERSION {A.HS_ABI_VERSION}u" in src
+    assert "hs_launch_info;      /* 32 bytes */" in src and C.sizeof(A.LaunchInfo) == 32
+
+
+def test_a_library_of_another_abi_version_fails_the_version_check(tmp_path):
+    """A library built from older sources exports an older hs_version and lacks newer entry points: loading it names
+    the version mismatch, not the first missing symbol."""
+    import shutil
+    import subprocess
+    cc = shutil.which(os.environ.get("CC", "cc")) or shutil.which("gcc")
+    if cc is None:
+        pytest.skip("no C compiler")
+    src = tmp_path / "stale.c"
+    src.write_text(f"unsigned int hs_version(void) {{ return {A.HS_ABI_VERSION - 1}u; }}\n")
+    so = tmp_path / "libstale.so"
+    subprocess.check_call([cc, "-shared", "-fPIC", "-o", str(so), str(src)])
+    with pytest.raises(engine.EngineError, match=f"ABI version {A.HS_ABI_VERSION - 1}, this package needs {A.HS_ABI_VERSION}"):
+        engine.load_library(str(so))
 
 
 def test_engine_fails_loudly_without_a_gpu(lib):
