@@ -620,7 +620,8 @@ static void orun_finish(orun *Rp)
 {
 #define R (*Rp)
     const hs_outputs *out = R.out; const uint32_t r = R.r; const uint32_t ne = R.m->n_entities;
-    const int64_t processed = R.processed; const uint64_t h = R.hash;
+    /* with the hash off the summary holds 0, as on every engine -- also for a replica that has processed no event */
+    const int64_t processed = R.processed; const uint64_t h = (R.p->flags & HS_RUN_ORDER_HASH) ? R.hash : 0;
     if (out->summaries) {
         hs_replica_summary *s = &out->summaries[r];
         s->events_processed = processed; s->final_time_ns = R.now; s->order_hash = h;

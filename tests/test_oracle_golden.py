@@ -50,3 +50,13 @@ def test_reference_counter_kat():
     got = O.oracle_run(model, O.make_params(**kw))
     st = got["entity_stats"][0]
     assert int(st[0]["c0"]) == 61 and int(st[1]["c0"]) == 60
+
+
+def test_order_hash_off_is_zero_even_before_the_first_event():
+    """With HS_RUN_ORDER_HASH off every engine reports order_hash 0; so must the oracle for a replica paused before
+    it has processed any event (its hash never left HS_HASH_INIT)."""
+    import happysim_b200 as hs
+    s = O.oracle_run(hs.mm1(rate=0.5), O.make_params(seed=3, end_ns=10**10, window_end_ns=10**9, n_replicas=64,
+                                                      flags=0))["summaries"]
+    assert (s["events_processed"] == 0).any() and (s["events_processed"] > 0).any()
+    assert (s["order_hash"] == 0).all()
