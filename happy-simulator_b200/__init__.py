@@ -23,6 +23,7 @@ from .api import (  # noqa: F401,E402
     Server, ServerStats, CachingServer, CachingServerStats, Sink, Counter, LoadBalancer, LoadBalancerStats, RoundRobin, ConsistentHash,
     UniformKeyContext, ZipfKeyContext, StepProfile, Simulation, SimulationSummary, EntitySummary, QueueStats, ParallelRunner, RunConfig,
     ParallelResult, seed, run_lowered, LinearRampProfile, SpikeProfile,
+    FaultSchedule, CrashNode, PauseNode, FaultHandle, FaultStats,
 )
 from . import api  # noqa: F401,E402
 from .instrumentation import Data, BucketedData, LatencyTracker, ThroughputTracker, Probe  # noqa: F401,E402

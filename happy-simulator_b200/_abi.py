@@ -3,13 +3,14 @@ from __future__ import annotations
 
 import ctypes as C
 
-HS_ABI_VERSION = 5
+HS_ABI_VERSION = 6
 
 HS_OK, HS_ERR_INVALID, HS_ERR_CUDA, HS_ERR_NO_DEVICE, HS_ERR_STATE, HS_ERR_OVERFLOW = 0, -1, -2, -3, -4, -5
 
 HS_ENT_SOURCE, HS_ENT_SERVER, HS_ENT_SINK, HS_ENT_COUNTER, HS_ENT_LB, HS_ENT_PROBE, HS_ENT_SKETCH = 1, 2, 3, 4, 5, 6, 7
 HS_ENT_CACHE_SERVER = 8
 HS_ENT_REMOTE = 9
+HS_ENT_FAULT = 10
 HS_SK_HLL, HS_SK_CMS, HS_SK_BLOOM, HS_SK_TOPK, HS_SK_TDIGEST, HS_SK_RESERVOIR = 1, 2, 3, 4, 5, 6
 METRICS = {"depth": 0, "active_requests": 1, "utilization": 2, "available_capacity": 3, "stats_accepted": 4,
            "stats_dropped": 5, "events_received": 6, "total": 7, "generated_count": 8}
@@ -21,16 +22,17 @@ HS_PROF_CONSTANT, HS_PROF_LINEAR_RAMP, HS_PROF_SPIKE, HS_PROF_STEP = 0, 1, 2, 3
 
 (HS_EV_SOURCE_TICK, HS_EV_REQ_LB, HS_EV_REQ_ENQUEUE, HS_EV_NOTIFY, HS_EV_POLL, HS_EV_DELIVER,
  HS_EV_REQ_WORKER, HS_EV_CONTINUATION, HS_EV_REQ_SINK, HS_EV_LB_RESPONSE, HS_EV_REQ_COUNTER,
- HS_EV_PROBE, HS_EV_REQ_SKETCH) = range(13)
+ HS_EV_PROBE, HS_EV_REQ_SKETCH, HS_EV_FAULT) = range(14)
 
 EVENT_KIND_NAMES = ["SOURCE_TICK", "REQ_LB", "REQ_ENQUEUE", "NOTIFY", "POLL", "DELIVER",
-                    "REQ_WORKER", "CONTINUATION", "REQ_SINK", "LB_RESPONSE", "REQ_COUNTER", "PROBE", "REQ_SKETCH"]
+                    "REQ_WORKER", "CONTINUATION", "REQ_SINK", "LB_RESPONSE", "REQ_COUNTER", "PROBE", "REQ_SKETCH", "FAULT"]
 
 HS_ST_QUEUE_OVERFLOW, HS_ST_FEL_OVERFLOW, HS_ST_REJECT_PATH, HS_ST_TRACE_EXHAUSTED, HS_ST_EVENT_LIMIT = 1, 2, 4, 8, 16
 HS_ST_SKETCH_OVERFLOW = 32
 HS_RUN_LINKED = 4
 HS_ST_LINK_OVERFLOW = 64
 HS_ST_LINK_TIE = 128
+HS_ST_FAULT_TIE = 256
 
 HS_STREAM_ARRIVAL, HS_STREAM_SERVICE, HS_STREAM_ROUTING, HS_STREAM_LINK_LOSS, HS_STREAM_LINK_LATENCY = 0, 1, 2, 3, 4
 

@@ -24,7 +24,7 @@ import numpy as np
 from . import _abi as A
 from . import lowering
 from .engine import Engine, make_params
-from .results import EntitySummary, QueueStats, SimulationSummary, replica_summary, write_back  # noqa: F401
+from .results import EntitySummary, QueueStats, SimulationSummary, fault_cancelled, replica_summary, write_back  # noqa: F401
 
 default_seed = 0
 
@@ -572,6 +572,110 @@ class LoadBalancer(Entity):
                                  requests_forwarded=self._requests_forwarded)
 
 
+# ----------------------------------------------------------------------------- faults/ (node faults)
+@dataclass(frozen=True)
+class FaultStats:
+    """faults/fault.py:95-108"""
+    faults_scheduled: int
+    faults_activated: int
+    faults_deactivated: int
+    faults_cancelled: int
+
+
+class _FaultEvent:
+    """What the device needs of a fault's Event.once (core/event.py:372-401): its time, its sort index and the
+    ``_cancelled`` flag FaultHandle.cancel() sets."""
+
+    def __init__(self, time: Instant, sort_index: int):
+        self.time, self._sort_index, self._cancelled = time, sort_index, False
+
+    def cancel(self) -> None:
+        self._cancelled = True
+
+
+class FaultHandle:
+    """faults/fault.py:55-87: cancel() before run() cancels the events the schedule has generated so far (a
+    Simulation generates them when it is built)."""
+
+    def __init__(self, fault):
+        self.fault = fault
+        self._events: list = []
+        self._cancelled = False
+
+    @property
+    def cancelled(self) -> bool:
+        return self._cancelled
+
+    def cancel(self) -> None:
+        if self._cancelled:
+            return
+        self._cancelled = True
+        for ev in self._events:
+            ev.cancel()
+
+
+@dataclass(frozen=True)
+class CrashNode:
+    """faults/node_faults.py:16-78: crash ``entity_name`` at ``at`` s, restart at ``restart_at`` s (None: never)."""
+    entity_name: str
+    at: float
+    restart_at: float | None = None
+
+
+@dataclass(frozen=True)
+class PauseNode:
+    """faults/node_faults.py:81-128: pause ``entity_name`` from ``start`` s to ``end`` s."""
+    entity_name: str
+    start: float
+    end: float
+
+
+def _start_schedule(schedule, sources, entities, probes) -> None:
+    """Generate the events of ``schedule`` (the mirror's or the reference's FaultSchedule) onto its handles, as
+    FaultSchedule.start does when a Simulation is built: names resolve (KeyError otherwise), faults other than
+    CrashNode / PauseNode raise UnsupportedModelError, and the sort indices follow the sources' and probes' first
+    ticks.  A FaultHandle.cancel() from then on marks these events."""
+    lowering.fault_events(schedule, sources, entities, probes)      # names and fault classes, before anything changes
+    for h in schedule._handles:
+        h._events = []
+    k = len(list(sources or [])) + len(list(probes or []))
+    for fault, h in zip(schedule._faults, schedule._handles):
+        times = [fault.at] + ([] if fault.restart_at is None else [fault.restart_at]) \
+            if type(fault).__name__ == "CrashNode" else [fault.start, fault.end]
+        for t in times:
+            h._events.append(_FaultEvent(Instant.from_seconds(t), k))
+            k += 1
+
+
+class FaultSchedule:
+    """faults/schedule.py:29-135: ``add()`` node faults; the Simulation generates their events when it is built and
+    runs them on the device.  Only CrashNode and PauseNode run there."""
+
+    def __init__(self, name: str = "FaultSchedule"):
+        self.name = name
+        self._faults: list = []
+        self._handles: list[FaultHandle] = []
+        self._scheduled = 0
+
+    def add(self, fault) -> FaultHandle:
+        h = FaultHandle(fault)
+        self._faults.append(fault)
+        self._handles.append(h)
+        self._scheduled += 1
+        return h
+
+    def start(self, sources, entities, probes) -> None:
+        """FaultSchedule.start (schedule.py:64-96): every fault's events, with sort indices from the bootstrap
+        counter that the sources' and probes' first ticks started."""
+        _start_schedule(self, sources, entities, probes)
+
+    @property
+    def stats(self) -> FaultStats:
+        """The reference never counts activations or deactivations (they stay 0)."""
+        return FaultStats(faults_scheduled=self._scheduled, faults_activated=0, faults_deactivated=0,
+                          faults_cancelled=sum(1 for h in self._handles if h.cancelled))
+
+
 def stock_streams(seed: int, n_replicas: int, n_draws: int, seed_stride: int = 1):
     """The reference's two process-global MT19937 streams as unit-rate exponential variates:
     row r is what ``random.seed(seed + r*seed_stride); numpy.random.seed(seed + r*seed_stride)`` yields.
@@ -613,9 +717,8 @@ class Simulation:
             raise ValueError("Cannot specify both 'duration' and 'end_time'")
         if start_time is not None and start_time.nanoseconds != 0:
             raise lowering.UnsupportedModelError("start_time must be Instant.Epoch on the device engine")
-        for nm, v in (("trace_recorder", trace_recorder), ("fault_schedule", fault_schedule)):
-            if v:
-                raise lowering.UnsupportedModelError(f"{nm}= is outside the accelerated path (SURVEY.md section 8)")
+        if trace_recorder:
+            raise lowering.UnsupportedModelError("trace_recorder= is outside the accelerated path (SURVEY.md section 8)")
         self._start_time = Instant.Epoch
         if duration is not None:
             self._end_time = self._start_time + duration
@@ -636,9 +739,12 @@ class Simulation:
         self._queue_ring = int(queue_ring) if queue_ring else 0
         self.last_run_info: dict = {}
         self._summary: SimulationSummary | None = None
+        self._fault_schedule = fault_schedule
         if _lowered is None:
+            if fault_schedule is not None:      # Simulation.__init__ bootstraps the schedule (simulation.py:162-169)
+                _start_schedule(fault_schedule, self._sources, self._entities, self._probes)
             _lowered = (*lowering.lower(self._sources, self._entities, probes=self._probes,
-                                        horizon_s=self._end_time.to_seconds()), Instant)
+                                        horizon_s=self._end_time.to_seconds(), fault_schedule=fault_schedule), Instant)
         self.model, self.objects, self._instant_cls = _lowered
 
     @classmethod
@@ -704,6 +810,8 @@ class Simulation:
         unbounded) is handled per ``on_overflow``: "grow" re-runs the ensemble with doubled rings (fresh,
         unwindowed runs only), "raise" raises, "ignore" returns the flagged statuses to the caller."""
         eng = _engine(self._device)
+        if lowering.refresh_fault_cancellation(self.model) and not upload and not resume:
+            upload = True                   # a FaultHandle was cancelled since the last upload
         if upload:
             eng.upload(self.model)
         if not resume:
@@ -784,6 +892,8 @@ def _run_many(sims, *, seed: int, seed_stride: int, rid_base: int, rid_stride: i
     lead = sims[0]
     n = len(sims)
     eng = _engine(lead._device)
+    for sm in sims:                     # FaultHandle.cancel() may have been called since the Simulation was built
+        lowering.refresh_fault_cancellation(sm.model)
     model = lead.model
     if n > 1:
         import copy
@@ -859,7 +969,8 @@ def _run_many(sims, *, seed: int, seed_stride: int, rid_base: int, rid_stride: i
         write_back(sm.model, sm.objects, out, k, sm._instant_cls)
         sm.last_run_info = {"launches": launches, "wall_s": wall, "queue_ring": ring, "batched_with": n,
                             "device_ms_last_launch": eng.last_run_ms(), "status": int(summ[k]["status"])}
-        sm._summary = replica_summary(summ[k], wall, sm._entities)
+        sm._summary = replica_summary(summ[k], wall, sm._entities,
+                                      events_cancelled=fault_cancelled(sm.model, out["entity_stats"][k]))
         res.append(sm._summary)
     return res
 
@@ -886,7 +997,8 @@ def run_lowered(ref_sim, model=None, objects=None, *, seed: int | None = None, r
     reference's attributes ``_sources``, ``_entities``, ``_start_time``, ``_end_time``."""
     if model is None:
         model, objects = lowering.lower(ref_sim._sources, ref_sim._entities, probes=getattr(ref_sim, "_probes", None) or None,
-                                        horizon_s=float(int(ref_sim._end_time.nanoseconds)) / 1e9)
+                                        horizon_s=float(int(ref_sim._end_time.nanoseconds)) / 1e9,
+                                        fault_schedule=getattr(ref_sim, "_fault_schedule", None))
     sim = Simulation._from_lowered(model, objects, sources=ref_sim._sources, entities=ref_sim._entities,
                                    end_ns=ref_sim._end_time.nanoseconds, seed=seed, replica=replica, device=device,
                                    instant_cls=type(ref_sim._start_time))
@@ -926,7 +1038,8 @@ class _ReplicaResults:
         sim, s = self._sim, self.raw["summaries"][i]
         write_back(sim.model, sim.objects, self.raw, i, sim._instant_cls)
         return ParallelResult(name=f"replica_{i}", status=int(s["status"]),
-                              summary=replica_summary(s, self._wall, sim._entities))
+                              summary=replica_summary(s, self._wall, sim._entities,
+                                                      events_cancelled=fault_cancelled(sim.model, self.raw["entity_stats"][i])))
 
     def __getitem__(self, i):
         if isinstance(i, slice):
@@ -976,6 +1089,8 @@ class ParallelRunner:
             if cfg.seed is not None:
                 sim._seed = int(cfg.seed)
             sims.append(sim)
+        for sm in sims:                 # cancellations are part of the topology: read them before grouping
+            lowering.refresh_fault_cancellation(sm.model)
         res: list = [None] * len(sims)
         for g in _group_by_topology(sims):
             seeds = [sims[i]._seed for i in g]

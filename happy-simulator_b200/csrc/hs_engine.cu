@@ -107,6 +107,13 @@ static int validate_model(const hs_model_desc *m)
     if (m->n_entities == 0 || m->n_entities > 65535 || !m->entities) return fail(HS_ERR_INVALID, "n_entities must be 1..65535");
     uint32_t n = m->n_entities;
     int n_src = 0;
+    uint32_t n_fault = 0, n_remote = 0;
+    for (uint32_t i = 0; i < n; ++i) {
+        if (m->entities[i].kind == HS_ENT_REMOTE) n_remote++;
+        if (m->entities[i].kind == HS_ENT_FAULT) n_fault++;
+        else if (n_fault) return fail(HS_ERR_INVALID, "entity %u: FAULT rows must come after every other row", i);
+    }
+    if (n_fault && n_remote) return fail(HS_ERR_INVALID, "a model with REMOTE rows (a linked partition) cannot have FAULT rows");
     for (uint32_t i = 0; i < n; ++i) {
         const hs_entity_desc &e = m->entities[i];
         switch (e.kind) {
@@ -166,6 +173,16 @@ static int validate_model(const hs_model_desc *m)
             if (!(e.d0 > 0.0)) return fail(HS_ERR_INVALID, "entity %u: ttl must be > 0 (eviction_policies.py:174)", i);
             break;
         case HS_ENT_SINK: case HS_ENT_COUNTER: break;
+        case HS_ENT_FAULT: {
+            if (e.target < 0 || (uint32_t)e.target >= n) return fail(HS_ERR_INVALID, "entity %u: fault target out of range", i);
+            const int tk = m->entities[e.target].kind;
+            if (tk == HS_ENT_FAULT || tk == HS_ENT_REMOTE || tk == HS_ENT_PROBE)
+                return fail(HS_ERR_INVALID, "entity %u: a fault cannot target a FAULT, REMOTE or PROBE-measure row", i);
+            if (e.l0 < 0) return fail(HS_ERR_INVALID, "entity %u: negative fault time", i);
+            if ((e.i1 != 0 && e.i1 != 1) || (e.i2 != 0 && e.i2 != 1) || e.i3 < 0)
+                return fail(HS_ERR_INVALID, "entity %u: fault action and cancelled flag must be 0 or 1, the sort index >= 0", i);
+            break;
+        }
         case HS_ENT_REMOTE:
             if (e.i0 < 0 || e.i0 >= 16 || e.i1 < 0) return fail(HS_ERR_INVALID, "entity %u: REMOTE row needs a link slot in 0..15 and a destination entity id", i);
             if (m->outbox_cap == 0) return fail(HS_ERR_INVALID, "entity %u: a model with REMOTE rows needs outbox_cap > 0", i);
@@ -359,7 +376,7 @@ static int general_setup(hs_engine *E, const hs_kernel_run &R, bool thread, bool
     /* FEL slots: one pending SourceEvent per source, one ProcessContinuation per busy
      * server slot, plus the same-timestamp protocol events in flight. */
     uint64_t live = 24;
-    uint32_t n_servers = 0;
+    uint32_t n_servers = 0, n_faults = 0;
     bool any_profile = false;
     std::vector<int32_t> srv_index(ne, -1);
     for (uint32_t i = 0; i < ne; ++i) {
@@ -369,6 +386,7 @@ static int general_setup(hs_engine *E, const hs_kernel_run &R, bool thread, bool
         if (e.kind == HS_ENT_CACHE_SERVER) live += 64;      /* no concurrency limit: one pending continuation per request in service;
                                                               64 covers 10 000 requests/s through the ~6 ms of a miss (overflow is flagged) */
         if (e.kind == HS_ENT_SERVER || e.kind == HS_ENT_CACHE_SERVER) srv_index[i] = (int32_t)n_servers++;
+        if (e.kind == HS_ENT_FAULT) { live += 1; n_faults++; }      /* pending from the bootstrap until it fires */
     }
     live += E->inbox_cap;                            /* what a barrier can deliver is scheduled at once */
     const uint32_t S = (uint32_t)((live + 31) / 32) * 32;
@@ -400,8 +418,11 @@ static int general_setup(hs_engine *E, const hs_kernel_run &R, bool thread, bool
     M.n_entities = ne; M.n_cells = E->n_cells; M.n_servers = n_servers; M.fel_slots = S; M.block_bytes = block_bytes;
     M.n_backends = (uint32_t)E->backends.size(); M.model_bytes = 0;
     M.outbox_cap = E->outbox_cap; M.inbox_cap = E->inbox_cap;
-    M.fixed_slots = 0; M.pad_ = 0;
-    *fl = (want_hash ? HS_WF_HASH : 0) | (want_rec ? HS_WF_REC : 0) | (any_profile ? HS_WF_PROFILE : 0);
+    M.fixed_slots = 0; M.n_faults = n_faults;
+    /* a model with faults runs the FAULTS instantiations, which always include the profile path (half the kernels to
+     * build; with no profile row it is one untaken branch per tick) */
+    *fl = (want_hash ? HS_WF_HASH : 0) | (want_rec ? HS_WF_REC : 0) | (any_profile || n_faults ? HS_WF_PROFILE : 0) |
+          (n_faults ? HS_WF_FAULTS : 0);
     return HS_OK;
 }
 
@@ -426,9 +447,11 @@ static int launch_warp(hs_engine *E, const hs_kernel_run &R, const hs_kernel_out
     CUDA_TRY(cudaMemsetAsync(E->d_counter.p, 0, 16, E->stream));
     using kernel = void (*)(hs_warp_model, hs_kernel_run, unsigned char *, hs_wring_entry *, hs_kernel_out, unsigned int *);
     static const kernel kernels[] = {HS_K4(hs_warp_kernel, 0), HS_K4(hs_warp_kernel, 4)};
-    CUDA_TRY(cudaFuncSetAttribute(kernels[fl], cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
+    static const kernel fault_kernels[] = {HS_K4(hs_warp_kernel, HS_WF_FAULTS | HS_WF_PROFILE)};
+    const kernel kern = (fl & HS_WF_FAULTS) ? fault_kernels[fl & 3] : kernels[fl];
+    CUDA_TRY(cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
     const hs_launch_info info = {1, HS_KERNEL_WARP, (uint32_t)fl, 1, 0, grid, warps * 32, smem};
-    return timed_launch(E, info, kernels[fl], M, R, (unsigned char *)E->d_state.p,
+    return timed_launch(E, info, kern, M, R, (unsigned char *)E->d_state.p,
                         (hs_wring_entry *)E->d_rings.p, O, (unsigned int *)E->d_counter.p);
 }
 
@@ -467,14 +490,18 @@ static int launch_thread(hs_engine *E, hs_kernel_run R, const hs_kernel_out &O, 
                                      HS_K4(hs_thread_kernel, 12), HS_K4(hs_thread_kernel, 16), HS_K4(hs_thread_kernel, 20),
                                      HS_K4(hs_thread_kernel, 24), HS_K4(hs_thread_kernel, 28)};
     static const kernel wide_kernels[] = {HS_K4(hs_thread_kernel_wide, 0), HS_K4(hs_thread_kernel_wide, 4)};
+    static const kernel fault_kernels[] = {HS_K4(hs_thread_kernel, HS_WF_FAULTS | HS_WF_PROFILE),
+                                           HS_K4(hs_thread_kernel, HS_WF_FAULTS | HS_WF_HEAPTOP | HS_WF_PROFILE)};
+    static const kernel fault_wide_kernels[] = {HS_K4(hs_thread_kernel_wide, HS_WF_FAULTS | HS_WF_PROFILE)};
     /* small launches (every block resident at 4 blocks per SM, no shared-memory heap top, not linked): the spill-free
      * instantiation, see hs_thread_kernel_wide */
     const bool wide = !R.heap_top && !linked && tblocks <= (uint32_t)E->sm_count * HS_T_WIDE_BLOCKS;
     if (!wide) fl |= (R.heap_top ? HS_WF_HEAPTOP : 0) | (linked ? HS_WF_LINKED : 0);
     const hs_launch_info info = {3, wide ? (uint32_t)HS_KERNEL_THREAD_WIDE : (uint32_t)HS_KERNEL_THREAD, (uint32_t)fl,
                                  R.lane_stride, R.heap_top, tblocks, HS_THREAD_BLOCK, (uint32_t)dyn_smem};
-    return timed_launch(E, info, wide ? wide_kernels[fl] : kernels[fl], M, R, (unsigned char *)E->d_state.p,
-                        (hs_wring_entry *)E->d_rings.p, O);
+    const kernel kern = !(fl & HS_WF_FAULTS) ? (wide ? wide_kernels[fl] : kernels[fl])
+                      : wide ? fault_wide_kernels[fl & 3] : fault_kernels[(fl & 3) | ((fl & HS_WF_HEAPTOP) ? 4 : 0)];
+    return timed_launch(E, info, kern, M, R, (unsigned char *)E->d_state.p, (hs_wring_entry *)E->d_rings.p, O);
 }
 #undef HS_K4
 
@@ -636,6 +663,9 @@ int hs_run(hs_engine *E, const hs_run_params *p)
     if (engine == 0) engine = E->lane_ok && !linked ? 2 : 3;
     if (engine < 1 || engine > 3) return fail(HS_ERR_INVALID, "unknown engine %d", engine);
     if (linked && engine != 3) return fail(HS_ERR_INVALID, "linked partitions run on the thread engine (engine 3)");
+    const bool faults = std::any_of(E->ents.begin(), E->ents.end(), [](const hs_entity_desc &e) { return e.kind == HS_ENT_FAULT; });
+    if (faults && linked) return fail(HS_ERR_INVALID, "a linked partition cannot have FAULT rows (fault schedules)");
+    if (engine == 2 && faults) return fail(HS_ERR_INVALID, "the lane engine does not run fault schedules (the model has FAULT rows): use engine 0, 1 or 3");
     if (engine == 2 && !E->lane_ok) return fail(HS_ERR_INVALID, "lane engine needs Source -> Server(concurrency <= 64) -> Sink|Counter");
 
     const uint32_t ring = p->queue_ring ? pow2_at_least(p->queue_ring) : engine == 2 ? 256 : 128;

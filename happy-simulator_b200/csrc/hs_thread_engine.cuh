@@ -217,6 +217,20 @@ hs_thread_body(const hs_warp_model &M, const hs_kernel_run &P, unsigned char *__
                             if (!HS_T_LT(nk.time, nk.k2, q.time, q.k2)) break; kstore(k, q); k = p; }
             kstore(k, nk);
         }
+        /* FaultSchedule.start() after the sources and probes (simulation.py:162-169): one Event.once per fault event, its
+         * sort index taken from the same global counter (carried in the row); with entity-owned slots the row owns its slot */
+        if (FLAGS & HS_WF_FAULTS)
+            for (uint32_t i = ne - M.n_faults; i < ne; ++i) {
+                if (hn >= S) { hdr.status |= HS_ST_FEL_OVERFLOW; break; }
+                const uint32_t slot = M.fixed_slots ? i : FREE[S - hn - 1];
+                hs_tpay pp; pp.created = 0; pp.aux = 0ull; pp.m0 = HS_EV_FAULT | (i << 8); pp.key = -1; pp.hook = 0u; pp.pad = 0u;
+                *pay_at(slot) = pp;
+                hs_tkey nk; nk.time = ENTS[i].l0; nk.k2 = ((uint64_t)(uint32_t)ENTS[i].i3 << 16) | slot;
+                uint32_t k = hn++;
+                while (k > 0) { const uint32_t p = (k - 1) >> HS_T_SHIFT; const hs_tkey q = kload(p);
+                                if (!HS_T_LT(nk.time, nk.k2, q.time, q.k2)) break; kstore(k, q); k = p; }
+                kstore(k, nk);
+            }
         h_fel = (int32_t)hn;
         hdr.free_top = hn;                               /* free_top holds the heap size in this engine */
         hdr.ctr = 0;
@@ -302,7 +316,13 @@ hs_thread_body(const hs_warp_model &M, const hs_kernel_run &P, unsigned char *__
         fkey.k2 |= slot;
         return true;
     };
+    /* an event created during the run that ties with a pending FAULT event (HS_ST_FAULT_TIE) */
+    auto fault_tie = [&](const int64_t t, const uint64_t idx) {
+        if (hs_fault_tie(ENTS, ne, M.n_faults, t, idx, (const unsigned char *)&E[0].w, (uint32_t)sizeof(hs_tent)))
+            hdr.status |= HS_ST_FAULT_TIE;
+    };
     auto heap_push_key = [&](const hs_tkey fkey) {                       /* the key sifts up */
+        if (FLAGS & HS_WF_FAULTS) fault_tie(fkey.time, fkey.k2 >> 16);
         uint32_t k = heap_n++;
         while (k > 0) {
             const uint32_t p = (k - 1) >> HS_T_SHIFT;
@@ -385,6 +405,7 @@ hs_thread_body(const hs_warp_model &M, const hs_kernel_run &P, unsigned char *__
             went_u xs; went_load((int)ent, xs); hs_went *Xs = &xs.w;
             went_u xl; hs_went *Xl = &xl.w;
             if (d1.kind == HS_ENT_LB) went_load(t1, xl);             /* issued together with the source's: independent lines */
+            if ((FLAGS & HS_WF_FAULTS) && (Xs->crashed || (d1.kind == HS_ENT_LB && Xl->crashed))) return false;   /* dropped: generic path */
             const int64_t cur_ns = Xs->u.src.cur_ns; const uint64_t arr_draws = Xs->u.src.arr_draws, key_draws = Xs->u.src.key_draws;
             int32_t key = -1;
             if (ds.i1 > 0) key = hs_routing_key(hs_uniform(seed, rid, HS_STREAM_ROUTING | (ent << 8), key_draws), ds.i1,
@@ -408,6 +429,7 @@ hs_thread_body(const hs_warp_model &M, const hs_kernel_run &P, unsigned char *__
             if ((FLAGS & HS_WF_PROFILE) && ds.i3 > 0) nt = hs_next_arrival_profile_ns(&M.profiles[ds.i3 - 1], cur_ns, target);
             else nt = hs_next_arrival_ns(cur_ns, target, Xs->d0);
             if (nt == HS_T_EXHAUSTED || nt <= now) return false;
+            if ((FLAGS & HS_WF_FAULTS) && Xv->crashed) return false;
             const uint32_t q_head = Xv->u.srv.q_head, q_len = Xv->u.srv.q_len; const int32_t active = Xv->u.srv.active;
             const int32_t c_lim = Xv->i0;
             if (q_len >= P.ring) return false;
@@ -499,6 +521,7 @@ hs_thread_body(const hs_warp_model &M, const hs_kernel_run &P, unsigned char *__
             const int tgt = dv.target;
             int tkind = 0;
             if (tgt >= 0) { tkind = ENTS[tgt].kind; if (tkind != HS_ENT_SINK && tkind != HS_ENT_COUNTER) return false; }
+            if ((FLAGS & HS_WF_FAULTS) && tgt >= 0 && E[tgt].w.crashed) return false;   /* the sink drops the request: generic path */
             went_u xv; went_load((int)ent, xv); hs_went *Xv = &xv.w;
             if (tgt >= 0) hs_prefetch(&E[tgt]);     /* the sink's line: wanted after the draw */
             const uint32_t q_head = Xv->u.srv.q_head, q_len = Xv->u.srv.q_len;
@@ -623,6 +646,7 @@ hs_thread_body(const hs_warp_model &M, const hs_kernel_run &P, unsigned char *__
         if ((FLAGS & HS_WF_LINKED) && (KIND) == HS_EV_REQ_ANY && M.outbox_cap && ENTS[(ENT)].kind == HS_ENT_REMOTE)                \
             outbox_send((IDX), (CREATED), (KEY), (uint32_t)(ENT), now);                                  \
         else if (t_ <= now) {                                                                                 \
+            if (FLAGS & HS_WF_FAULTS) fault_tie(t_, (uint64_t)(IDX));                                    \
             if (now_n >= HS_W_NCAP) hdr.status |= HS_ST_FEL_OVERFLOW;                                    \
             else { hs_wnow n_; n_.time = t_; n_.idx = (IDX); n_.created = (CREATED); n_.aux = (AUX);     \
                    n_.m0 = (uint32_t)(KIND) | ((uint32_t)(ENT) << 8); n_.key = (KEY); n_.hook = (HOOK); n_.pad = 0u; \
@@ -720,7 +744,11 @@ hs_thread_body(const hs_warp_model &M, const hs_kernel_run &P, unsigned char *__
             h_fel--;
             need_heap = false;
             int chain_done = 0;
-            if (ev.time < now0) chain_done = 1;          /* "time travel": skipped (simulation.py:479-489) */
+            if ((FLAGS & HS_WF_FAULTS) && (ev.m0 & 0xffu) == HS_EV_FAULT && ENTS[ev.m0 >> 8].i2) {
+                E[ev.m0 >> 8].w.u.flt.cancelled++;       /* a cancelled event: counted, not processed (simulation.py:475-477) */
+                chain_done = 1;
+            }
+            else if (ev.time < now0) chain_done = 1;     /* "time travel": skipped (simulation.py:479-489) */
             else if (fused_chain()) chain_done = 1;      /* the whole same-timestamp chain ran as straight-line code */
             else { int k = (int)(ev.m0 & 0xffu);
                    if (k == (int)HS_EV_REQ_ANY) {
@@ -741,11 +769,12 @@ hs_thread_body(const hs_warp_model &M, const hs_kernel_run &P, unsigned char *__
          * warp holds a single replica: 170 KB of code); `kind` is warp-uniform in every pass, so the switch inside
          * process() is a uniform branch and the lanes that take it run the same handler.
          * One nibble per pass, low first: TICK 0, CONTINUATION 7, PROBE 11, REQ_LB 1, ENQUEUE 2, SINK 8, COUNTER 10,
-         * SKETCH 12, NOTIFY 3, LB_RESPONSE 9, POLL 4, DELIVER 5, WORKER 6 (the HS_EV_* values of include/hs_b200.h) */
+         * SKETCH 12, NOTIFY 3, LB_RESPONSE 9, POLL 4, DELIVER 5, WORKER 6 (the HS_EV_* values of include/hs_b200.h), and
+         * with HS_WF_FAULTS a last pass for FAULT 13 */
         if (ev_kind < 0) continue;                   /* the fused chain did it all: nothing for the generic passes */
 #pragma unroll 1
-        for (int ph = 0; ph < 13; ++ph) {
-            const int kind = single ? ev_kind : (int)((0x65493ca821b70ull >> (4 * ph)) & 15ull);
+        for (int ph = 0; ph < ((FLAGS & HS_WF_FAULTS) ? 14 : 13); ++ph) {
+            const int kind = single ? ev_kind : (int)((((FLAGS & HS_WF_FAULTS) ? 0xd65493ca821b70ull : 0x65493ca821b70ull) >> (4 * ph)) & 15ull);
             if (alive && ev_kind >= 0 && ev_kind == kind) { process(kind); next_event(); }
         }
     }
@@ -775,7 +804,7 @@ hs_thread_body(const hs_warp_model &M, const hs_kernel_run &P, unsigned char *__
         O.summaries[r] = s;
     }
     if (O.stats)
-        for (uint32_t i = 0; i < ne; ++i) O.stats[(size_t)r * ne + i] = hs_went_stats(&E[i].w, ENTS[i].kind);
+        for (uint32_t i = 0; i < ne; ++i) O.stats[(size_t)r * ne + i] = hs_went_stats_f<FLAGS>(&E[i].w, ENTS[i].kind);
 }
 
 /* Two entry points around the one body.  hs_thread_kernel: 128 registers per thread, 8 blocks of 64 threads per SM -- the

@@ -39,6 +39,8 @@
 #define HS_WF_HEAPTOP 8    /* thread engine: the heap's top levels live in shared memory (launches with several replicas per warp) */
 #define HS_WF_LINKED 16    /* thread engine: a partition of a linked ParallelSimulation (REMOTE rows -> outbox, inbox drained at
                               launch, finished replicas run on, tie detection); compiled out of every other launch */
+#define HS_WF_FAULTS 32    /* the model has FAULT rows (node faults): their bootstrap, the crashed-entity drop, cancelled pops and
+                              the tie test; compiled out of every other launch */
 
 struct __align__(16) hs_warp_hdr {      /* 128 B */
     int64_t now; uint64_t ctr; int64_t processed; uint64_t hash;
@@ -53,7 +55,8 @@ struct __align__(16) hs_went {          /* 96 B per entity */
     double d0;          /* effective rate / mean (cell override applied)          */
     double lambda;      /* SERVER: 1 / mean (exponential.py:36)                   */
     int32_t i0;         /* effective concurrency / arrival kind / strategy        */
-    int32_t pad0; int64_t pad1;
+    int32_t crashed;    /* Entity._crashed (faults/node_faults.py), set and cleared by FAULT events */
+    int64_t pad1;
     union {
         struct { int64_t cur_ns; uint64_t arr_draws, key_draws; int64_t generated, provider; } src;
         struct { uint32_t q_head, q_len; int32_t active, pad; uint64_t svc_draws;
@@ -61,6 +64,7 @@ struct __align__(16) hs_went {          /* 96 B per entity */
         struct { int64_t received; double sum, comp, sumsq, mn, mx; } snk;
         struct { uint64_t rr_index; int64_t received, forwarded, in_flight, responses; } lb;
         struct { int64_t processed, added; } sk;
+        struct { int64_t fired, cancelled; } flt;   /* FAULT: events fired / popped while cancelled */
         uint64_t raw[8];
     } u;
 };
@@ -85,7 +89,7 @@ struct hs_warp_model {
     uint32_t block_bytes;           /* bytes of one replica block (multiple of 16)          */
     uint32_t n_backends, model_bytes; /* shared-memory copy of the model tables (per CTA)     */
     uint32_t outbox_cap, inbox_cap;   /* linked partitions (HS_ENT_REMOTE rows / link destination), else 0 */
-    uint32_t fixed_slots, pad_;       /* thread engine: every entity has at most ONE pending future event (sources: the next
+    uint32_t fixed_slots, n_faults;   /* n_faults: FAULT rows, the last n_faults entities of the model.  fixed_slots: thread engine: every entity has at most ONE pending future event (sources: the next
                                          tick; servers with concurrency 1: the continuation), so its payload slot is its
                                          entity id -- no free-slot stack traffic on the heap's push / pop path */
 };
@@ -126,6 +130,30 @@ __device__ __forceinline__ hs_entity_stats hs_went_stats(const hs_went *e, int32
     case HS_ENT_SKETCH: a.c0 = e->u.sk.processed; a.c1 = e->u.sk.added; break;
     }
     return a;
+}
+/* hs_went_stats of an instantiation that may hold FAULT rows (c0 fired, c1 popped while cancelled) */
+template <int FLAGS>
+__device__ __forceinline__ hs_entity_stats hs_went_stats_f(const hs_went *e, int32_t kind)
+{
+    if ((FLAGS & HS_WF_FAULTS) && kind == HS_ENT_FAULT) {
+        hs_entity_stats a; a.c0 = e->u.flt.fired; a.c1 = e->u.flt.cancelled; a.c2 = a.c3 = 0; a.f0 = a.f1 = a.f2 = a.f3 = 0.0;
+        return a;
+    }
+    return hs_went_stats(e, kind);
+}
+
+/* An event created during the run with the key (t, idx) of a FAULT event that is still pending (neither fired nor popped
+ * cancelled): heapq would order the pair by its array layout (HS_ST_FAULT_TIE).  The FAULT rows are the model's last
+ * n_faults rows, their keys are (l0, i3); row i's hs_went is at base + i * stride bytes. */
+__device__ __forceinline__ bool hs_fault_tie(const hs_entity_desc *ENTS, uint32_t ne, uint32_t nf, int64_t t, uint64_t idx,
+                                             const unsigned char *base, uint32_t stride)
+{
+    for (uint32_t i = ne - nf; i < ne; ++i)
+        if (ENTS[i].l0 == t && (uint64_t)(uint32_t)ENTS[i].i3 == idx) {
+            const hs_went *f = (const hs_went *)(base + (size_t)i * stride);
+            if (f->u.flt.fired == 0 && f->u.flt.cancelled == 0) return true;
+        }
+    return false;
 }
 
 /* ---- PTX helpers: mbarrier + TMA 1-D bulk copies ------------------------- */
@@ -282,6 +310,15 @@ hs_warp_kernel(hs_warp_model M, hs_kernel_run P, unsigned char *__restrict__ blo
                     f_time[sl] = e->u.src.cur_ns; f_idx[sl] = boot++; f_m0[sl] = HS_EV_SOURCE_TICK | (i << 8);
                     f_key[sl] = -1; f_hook[sl] = 0; nf++;
                 }
+                /* FaultSchedule.start() after the sources and probes (simulation.py:162-169): one Event.once per fault
+                 * event, its sort index taken from the same global counter (carried in the row) */
+                if (FLAGS & HS_WF_FAULTS)
+                    for (uint32_t i = ne - M.n_faults; i < ne; ++i) {
+                        if (H->free_top == 0) { H->status |= HS_ST_FEL_OVERFLOW; break; }
+                        const uint32_t sl = f_free[--H->free_top];
+                        f_time[sl] = ENTS[i].l0; f_idx[sl] = (uint64_t)(uint32_t)ENTS[i].i3; f_m0[sl] = HS_EV_FAULT | (i << 8);
+                        f_key[sl] = -1; f_hook[sl] = 0; f_created[sl] = 0; f_aux[sl] = 0ull; nf++;
+                    }
                 H->fel_n = nf; H->ctr = 0;
             }
             __syncwarp();
@@ -342,6 +379,10 @@ hs_warp_kernel(hs_warp_model M, hs_kernel_run P, unsigned char *__restrict__ blo
                     const hs_wnow ev = N[nb];
                     now_n--; N[nb] = N[now_n];
                     H->fel_n--;
+                    if ((FLAGS & HS_WF_FAULTS) && (ev.m0 & 0xffu) == HS_EV_FAULT && ENTS[ev.m0 >> 8].i2) {
+                        E[ev.m0 >> 8].u.flt.cancelled++;  /* a cancelled event: counted, not processed (simulation.py:475-477) */
+                        continue;
+                    }
                     if (ev.time < now0) continue;     /* "time travel": skipped (simulation.py:479-489) */
                     const int64_t now = ev.time;
                     const uint64_t bi = ev.idx;
@@ -366,6 +407,9 @@ hs_warp_kernel(hs_warp_model M, hs_kernel_run P, unsigned char *__restrict__ blo
 #define HS_W_PUSH(TIME, IDX, KIND, ENT, CREATED, AUX, KEY, HOOK)                                         \
     do {                                                                                                 \
         const int64_t t_ = (TIME);                                                                       \
+        if ((FLAGS & HS_WF_FAULTS) && hs_fault_tie(ENTS, ne, M.n_faults, t_, (uint64_t)(IDX),            \
+                                                   (const unsigned char *)E, (uint32_t)sizeof(hs_went))) \
+            H->status |= HS_ST_FAULT_TIE;                                                                \
         if (t_ <= now) {                                                                                 \
             if (now_n >= HS_W_NCAP) H->status |= HS_ST_FEL_OVERFLOW;                                     \
             else { hs_wnow n_; n_.time = t_; n_.idx = (IDX); n_.created = (CREATED); n_.aux = (AUX);     \
@@ -421,7 +465,7 @@ hs_warp_kernel(hs_warp_model M, hs_kernel_run P, unsigned char *__restrict__ blo
         }
         __syncwarp();
         if (O.stats)
-            for (uint32_t i = lane; i < ne; i += 32) O.stats[(size_t)r * ne + i] = hs_went_stats(&E[i], ENTS[i].kind);
+            for (uint32_t i = lane; i < ne; i += 32) O.stats[(size_t)r * ne + i] = hs_went_stats_f<FLAGS>(&E[i], ENTS[i].kind);
         hs_fence_async_smem();
         __syncwarp();
         if (lane == 0) hs_tma_store_1d(gblk, blk, M.block_bytes);

@@ -3,7 +3,8 @@
 After ``install()`` an unchanged reference script (``from happysimulator import Simulation, Source, ...``) runs
 its ``Simulation(...).run()`` on the device whenever its object graph lowers (lowering.py) and falls through to the
 reference's Python loop, untouched, when it does not (user-defined entities, auto-termination, tracing, the debugger
-control surface, fault schedules, a start time other than the epoch): nothing is ever mis-simulated.
+control surface, a start time other than the epoch, faults other than CrashNode / PauseNode): nothing is ever
+mis-simulated.  A fault schedule of node faults lowers to FAULT rows: the crash flag and its drop run on the device.
 
 What is patched (reference paths under happysimulator/):
   core/simulation.py:66   Simulation.__init__   wrapped only to snapshot numpy's global generator BEFORE the
@@ -50,8 +51,6 @@ def _eligible(sim):
         return "start_time other than Instant.Epoch"
     if sim._tracing_enabled:
         return "trace_recorder"
-    if sim._fault_schedule is not None:
-        return "fault_schedule"
     if sim._control is not None or sim._is_running or sim._event_router is not None or sim._pre_run_event_specs:
         return "control surface / re-entrant run / partition router / scheduled pre-run events"
     return None
@@ -98,7 +97,7 @@ def install(*, device: int = 0, verbose: bool = False) -> None:
                                      total_dropped=v.queue_stats.total_dropped))
                 for k, v in sm.entities.items()}
         return SimulationSummary(duration_s=sm.duration_s, total_events_processed=sm.total_events_processed,
-                                 events_cancelled=0, events_per_second=sm.events_per_second,
+                                 events_cancelled=sm.events_cancelled, events_per_second=sm.events_per_second,
                                  wall_clock_seconds=sm.wall_clock_seconds, entities=ents)
 
     def run(self):
@@ -108,7 +107,8 @@ def install(*, device: int = 0, verbose: bool = False) -> None:
         if why is None:
             try:
                 model, objects = lowering.lower(self._sources, self._entities, probes=self._probes or None,
-                                                horizon_s=float(int(self._end_time.nanoseconds)) / 1e9)
+                                                horizon_s=float(int(self._end_time.nanoseconds)) / 1e9,
+                                                fault_schedule=self._fault_schedule)
             except lowering.UnsupportedModelError as e:
                 why = str(e)
         if why is not None:
@@ -152,7 +152,8 @@ def install(*, device: int = 0, verbose: bool = False) -> None:
             if why is not None:
                 raise lowering.UnsupportedModelError(why)
             model, objects = lowering.lower(ref_sim._sources, ref_sim._entities, probes=ref_sim._probes or None,
-                                            horizon_s=float(int(ref_sim._end_time.nanoseconds)) / 1e9)
+                                            horizon_s=float(int(ref_sim._end_time.nanoseconds)) / 1e9,
+                                            fault_schedule=ref_sim._fault_schedule)
         except lowering.UnsupportedModelError as e:
             st["fallbacks"] += 1
             st["last_fallback_reason"] = str(e)

@@ -269,17 +269,60 @@ def _queue_policy(q):
     return (A.HS_Q_LIFO if name == "LIFOQueue" else A.HS_Q_FIFO), cap
 
 
+def fault_events(fault_schedule, sources, entities, probes):
+    """The node-fault events of ``fault_schedule`` (the reference's faults.FaultSchedule or the mirror's), in bootstrap
+    order: a list of (target object, time_ns, crash, sort_index, event).  ``event`` is the Event (or the mirror's
+    stand-in) whose ``_cancelled`` flag a FaultHandle.cancel() sets; it is read again when the model runs.
+
+    Names resolve as FaultSchedule._build_context does (faults/schedule.py:112-135): the ``.name`` of every object in
+    entities, sources and probes, in that order, the last one winning; an unknown name raises KeyError.  CrashNode
+    gives a crash event at ``at`` and, with ``restart_at``, a restart event; PauseNode a pause at ``start`` and a
+    resume at ``end`` (faults/node_faults.py:41-128).  Times and sort indices are those of the events the schedule
+    generated when the Simulation was built; a schedule that has not generated them yet gets the times
+    Instant.from_seconds gives and the indices that follow the sources' and probes' first ticks."""
+    by_name = {}
+    for o in list(entities or []) + list(sources or []) + list(probes or []):
+        by_name[getattr(o, "name", None)] = o
+    n_boot = len(list(sources or [])) + len(list(probes or []))
+    res = []
+    for fault, handle in zip(fault_schedule._faults, fault_schedule._handles):
+        cls = _cls(fault)
+        if cls == "CrashNode":
+            spec = [(fault.at, True)] + ([] if fault.restart_at is None else [(fault.restart_at, False)])
+        elif cls == "PauseNode":
+            spec = [(fault.start, True), (fault.end, False)]
+        else:
+            raise UnsupportedModelError(f"fault {cls}: only the node faults CrashNode and PauseNode run on the device "
+                                        "(network faults, ReduceCapacity and user-defined Fault classes do not)")
+        target = by_name[fault.entity_name]          # KeyError, as ctx.entities[name] raises it
+        evs = list(getattr(handle, "_events", []) or [])
+        for k, (t_s, crash) in enumerate(spec):
+            ev = evs[k] if k < len(evs) else None
+            if ev is not None:
+                t_ns, idx = int(ev.time.nanoseconds), int(ev._sort_index)
+            else:
+                t_ns = t_s * 1_000_000_000 if isinstance(t_s, int) else int(t_s * 1_000_000_000)   # Instant.from_seconds
+                idx = n_boot
+            n_boot = idx + 1
+            res.append((target, t_ns, crash, idx, ev))
+    return res
+
+
 def lower(sources, entities, *, key_population: int | None = None, probes=None, horizon_s: float | None = None,
-          remote: dict | None = None):
+          remote: dict | None = None, fault_schedule=None):
     """-> (FlatModel, objects) where objects[i] is the Python object of entity id i.
 
     ``remote``: {id(object): link slot} for objects that live in ANOTHER partition of a ParallelSimulation: a Server
     may name one as its downstream; it becomes an HS_ENT_REMOTE row (its destination entity id is filled in by the
     caller once the other partition is lowered, parallel.py).
 
+    ``fault_schedule``: a FaultSchedule of CrashNode / PauseNode faults (see ``fault_events``); every fault event
+    becomes an HS_ENT_FAULT row, after all other rows, with its cancelled flag as it is now.
+
     Entity ids: sources first (in ``sources`` order, the bootstrap order of
     Simulation.__init__), then every entity reachable from them, in ``entities`` order
     first and discovery order after."""
+    faults = fault_events(fault_schedule, sources, entities, probes) if fault_schedule is not None else []
     objs: list = []
     ids: dict[int, int] = {}
 
@@ -492,6 +535,28 @@ def lower(sources, entities, *, key_population: int | None = None, probes=None, 
     for sid, name, tgt, metric in probe_rows:
         pid = b._add(name + ".measure", A.HS_ENT_PROBE, tgt, A.METRICS[metric])
         b.set_target(sid, pid)
+    for tgt, t_ns, crash, idx, ev in faults:
+        if id(tgt) not in ids:
+            raise UnsupportedModelError(f"fault on {getattr(tgt, 'name', tgt)!r}: the entity is not part of the model")
+        b.fault(f"fault:{getattr(tgt, 'name', '?')}", target=ids[id(tgt)], time_ns=t_ns, crash=crash, sort_index=idx,
+                cancelled=bool(getattr(ev, "_cancelled", False)))
     model = b.build()
+    if faults:
+        model.fault_events = [ev for *_, ev in faults]
     # a source whose key population is set needs the table length to match (validated by the C-ABI too)
     return model, objs
+
+
+def refresh_fault_cancellation(model) -> bool:
+    """Copy the ``_cancelled`` flags of the model's fault events into its FAULT rows: FaultHandle.cancel() may be
+    called between building the Simulation and running it (faults/fault.py:80-87).  Returns whether a row changed."""
+    evs = getattr(model, "fault_events", None)
+    if not evs:
+        return False
+    changed = False
+    for i, ev in zip(model.ids_of(A.HS_ENT_FAULT), evs):
+        v = 1 if getattr(ev, "_cancelled", False) else 0
+        if int(model.entities["i2"][i]) != v:
+            model.entities["i2"][i] = v
+            changed = True
+    return changed

@@ -31,6 +31,7 @@ class FlatModel:
     key_cdf: np.ndarray = field(default_factory=lambda: np.zeros(0, np.float64))
     outbox_cap: int = 0                       # linked partitions: cross-partition events a replica can emit per window
     inbox_cap: int = 0                        # ... and receive per barrier
+    fault_events: list | None = None          # FAULT rows: the fault events whose `_cancelled` flags are re-read at run time
 
     @property
     def n_entities(self) -> int:
@@ -359,6 +360,14 @@ class ModelBuilder:
             strat = A.HS_LB_KEY_TABLE
             self._key_table = np.asarray(key_table, dtype=np.int32)
         return self._add(name, A.HS_ENT_LB, -1, strat, off, len(backends))
+
+    def fault(self, name="Fault", *, target, time_ns, crash, sort_index, cancelled=False):
+        """One event of a node fault (HS_ENT_FAULT, faults/node_faults.py CrashNode / PauseNode): at ``time_ns`` it sets
+        (``crash``) or clears the crashed flag of entity ``target``.  ``sort_index`` is the event's bootstrap sort index
+        (sources, then probes, then the faults in schedule order); ``cancelled``: its FaultHandle was cancelled.  FAULT
+        rows must come after every other row."""
+        return self._add(name, A.HS_ENT_FAULT, int(target), 0, 1 if crash else 0, 1 if cancelled else 0, int(time_ns),
+                         i3=int(sort_index))
 
     def set_target(self, ent, target):
         r = list(self._rows[ent]); r[1] = int(target); self._rows[ent] = tuple(r)

@@ -143,6 +143,10 @@ class ParallelSimulation:
         self._simulations: dict[str, Simulation] = {}
         self._linked = None
         if self._links:
+            for p in partitions:
+                if p.fault_schedule is not None:
+                    raise UnsupportedModelError(f"partition {p.name!r}: fault schedules in linked partitions do not run "
+                                                "on the device (independent partitions do)")
             self._init_linked(start_time, end_time, duration, window_size)
             return
         for k, p in enumerate(partitions):

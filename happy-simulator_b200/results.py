@@ -132,6 +132,28 @@ def write_back(model, objects, out, r: int, instant_cls) -> None:
             o._requests_received, o._requests_forwarded = int(row["c0"]), int(row["c1"])
         elif k == A.HS_ENT_SKETCH:
             _write_back_sketch(model, o, i, row, out, r)
+    _write_back_crashed(model, objects, st)
+
+
+def _write_back_crashed(model, objects, st) -> None:
+    """Entity._crashed after the run: the action of the last FAULT event that fired on the entity (FAULT events fire
+    in (time, sort index) order); entities no fault event reached keep theirs."""
+    last = {}
+    for i in model.ids_of(A.HS_ENT_FAULT):
+        if int(st[i]["c0"]):
+            e = model.entities[i]
+            key = (int(e["l0"]), int(e["i3"]))
+            tgt = int(e["target"])
+            if tgt not in last or key > last[tgt][0]:
+                last[tgt] = (key, bool(int(e["i1"])))
+    for tgt, (_, crashed) in last.items():
+        objects[tgt]._crashed = crashed
+
+
+def fault_cancelled(model, st) -> int:
+    """SimulationSummary.events_cancelled of one replica (``st`` its entity stats): the FAULT events popped while
+    cancelled."""
+    return int(sum(int(st[i]["c1"]) for i in model.ids_of(A.HS_ENT_FAULT)))
 
 
 def _write_back_sketch(model, o, i: int, row, out, r: int) -> None:
@@ -186,11 +208,11 @@ def entity_summaries(entities) -> dict[str, EntitySummary]:
     return res
 
 
-def replica_summary(row, wall_s: float, entities) -> SimulationSummary:
+def replica_summary(row, wall_s: float, entities, events_cancelled: int = 0) -> SimulationSummary:
     """The SimulationSummary of one replica: its hs_replica_summary ``row``, the run's wall time and the summaries of
     ``entities`` (read after write_back has published the replica onto them)."""
     duration_s = float(int(row["final_time_ns"])) / 1_000_000_000
     ev = int(row["events_processed"])
-    return SimulationSummary(duration_s=duration_s, total_events_processed=ev, events_cancelled=0,
+    return SimulationSummary(duration_s=duration_s, total_events_processed=ev, events_cancelled=int(events_cancelled),
                              events_per_second=ev / duration_s if duration_s > 0 else 0.0,
                              wall_clock_seconds=wall_s, entities=entity_summaries(entities))

@@ -28,7 +28,7 @@
 extern "C" {
 #endif
 
-#define HS_ABI_VERSION 5u
+#define HS_ABI_VERSION 6u
 
 typedef enum hs_status {
     HS_OK = 0,
@@ -66,6 +66,17 @@ enum {
                             insertion times (seconds; 0 = not cached), in the hs_outputs.sketches region.
                             hs_entity_stats: c0 accepted, c1 dropped, c2 requests_processed, c3 cache_misses,
                             f0 cache_hits, f1 cache_size (as doubles)                                   */
+    HS_ENT_FAULT = 10,   /* one event of a node fault (faults/node_faults.py:16-128 CrashNode, PauseNode): an Event.once
+                            aimed at a CallbackEntity that sets (crash, pause) or clears (restart, resume) `_crashed` on
+                            the entity it names.  target = that entity, l0 = the event's time in ns (Instant.from_seconds),
+                            i1 = 1 set / 0 clear, i2 = 1 if its FaultHandle was cancelled before the run, i3 = its
+                            bootstrap sort index (global counter: sources, then probes, then the faults in schedule order).
+                            While an entity's flag is set, Event.invoke (core/event.py:261-262) drops the events aimed at it
+                            -- counted and clock-moving, but neither handler nor completion hooks run: SOURCE_TICK (the
+                            source is silent from then on), REQ_ENQUEUE, REQ_SINK, REQ_COUNTER, REQ_SKETCH, REQ_LB,
+                            LB_RESPONSE.  hs_entity_stats: c0 = fired, c1 = popped while cancelled (events_cancelled,
+                            core/simulation.py:475-477: not processed, the clock does not move).  Not in models with
+                            REMOTE rows; the lane engine does not run them                                  */
     HS_ENT_REMOTE = 9    /* stand-in for an entity that lives in ANOTHER partition of a ParallelSimulation
                             (parallel/simulation.py:31, parallel/routing.py:17-63): an event whose target is this row
                             is never scheduled here -- the partition's router puts it, with its send time, into the
@@ -108,7 +119,8 @@ enum {
     HS_EV_LB_RESPONSE = 9,  /* _lb_response -> LoadBalancer          load_balancer.py:435         */
     HS_EV_REQ_COUNTER = 10, /* Request -> Counter                    common.py:92                 */
     HS_EV_PROBE = 11,       /* probe_event -> measurement callback   instrumentation/probe.py:51  */
-    HS_EV_REQ_SKETCH = 12   /* Request -> SketchCollector            sketch_collector.py:79       */
+    HS_EV_REQ_SKETCH = 12,  /* Request -> SketchCollector            sketch_collector.py:79       */
+    HS_EV_FAULT = 13        /* fault callback (set / clear _crashed) node_faults.py:41-128; entity = the FAULT row */
 };
 
 typedef struct hs_entity_desc {
@@ -242,6 +254,10 @@ typedef struct hs_run_params {
                                      and sort index (the indices come from different partitions' counters).  The reference
                                      orders such a pair by the accident of heapq's array layout; the engines order it by
                                      their own heap's, so this replica's event order may differ from the reference's      */
+#define HS_ST_FAULT_TIE 256u      /* an event created during the run tied with a pending FAULT event on both time and sort
+                                     index (the fault's index comes from the bootstrap counter, the other's from the run's):
+                                     heapq orders such a pair by its array layout, the engines by their own heap's, so this
+                                     replica's event order may differ from the reference's                               */
 
 typedef struct hs_replica_summary {
     int64_t events_processed;  /* SimulationSummary.total_events_processed (simulation.py:553) */
