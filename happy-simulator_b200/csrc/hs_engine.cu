@@ -96,11 +96,15 @@ struct hs_engine {
     std::vector<int32_t> srv_index_host;        /* what d_srv_index holds */
     dev_buf d_outbox, d_outbox_n, d_inbox, d_inbox_n;
     uint32_t link_replicas = 0;                 /* replicas the outbox / inbox buffers are sized for */
+    bool partition = false;                     /* the model came through hs_partition_upload */
 };
 
 /* ---- validation ----------------------------------------------------------- */
 
-static int validate_model(const hs_model_desc *m)
+/* partition: the model is a partition of a linked run (hs_partition_upload / hs_partition_validate), where FAULT rows
+ * may sit next to REMOTE rows -- each partition's Simulation bootstraps its own fault schedule.  A model checked on its
+ * own (hs_model_validate, hs_model_upload) keeps refusing FAULT rows next to REMOTE rows. */
+static int validate_model(const hs_model_desc *m, bool partition = false)
 {
     if (!m) return fail(HS_ERR_INVALID, "model is NULL");
     if (m->abi_version != HS_ABI_VERSION) return fail(HS_ERR_INVALID, "abi_version %u != %u", m->abi_version, HS_ABI_VERSION);
@@ -113,7 +117,8 @@ static int validate_model(const hs_model_desc *m)
         if (m->entities[i].kind == HS_ENT_FAULT) n_fault++;
         else if (n_fault) return fail(HS_ERR_INVALID, "entity %u: FAULT rows must come after every other row", i);
     }
-    if (n_fault && n_remote) return fail(HS_ERR_INVALID, "a model with REMOTE rows (a linked partition) cannot have FAULT rows");
+    if (n_fault && n_remote && !partition)
+        return fail(HS_ERR_INVALID, "a model with REMOTE rows (a linked partition) has FAULT rows only as a partition of a linked run (hs_partition_upload)");
     for (uint32_t i = 0; i < n; ++i) {
         const hs_entity_desc &e = m->entities[i];
         switch (e.kind) {
@@ -490,8 +495,11 @@ static int launch_thread(hs_engine *E, hs_kernel_run R, const hs_kernel_out &O, 
                                      HS_K4(hs_thread_kernel, 12), HS_K4(hs_thread_kernel, 16), HS_K4(hs_thread_kernel, 20),
                                      HS_K4(hs_thread_kernel, 24), HS_K4(hs_thread_kernel, 28)};
     static const kernel wide_kernels[] = {HS_K4(hs_thread_kernel_wide, 0), HS_K4(hs_thread_kernel_wide, 4)};
+    /* [fl & 3 | HEAPTOP ? 4 : 0 | LINKED ? 8 : 0]: linked launches never take the wide kernel, so it has no linked form */
     static const kernel fault_kernels[] = {HS_K4(hs_thread_kernel, HS_WF_FAULTS | HS_WF_PROFILE),
-                                           HS_K4(hs_thread_kernel, HS_WF_FAULTS | HS_WF_HEAPTOP | HS_WF_PROFILE)};
+                                           HS_K4(hs_thread_kernel, HS_WF_FAULTS | HS_WF_HEAPTOP | HS_WF_PROFILE),
+                                           HS_K4(hs_thread_kernel, HS_WF_LINKED | HS_WF_FAULTS | HS_WF_PROFILE),
+                                           HS_K4(hs_thread_kernel, HS_WF_LINKED | HS_WF_FAULTS | HS_WF_HEAPTOP | HS_WF_PROFILE)};
     static const kernel fault_wide_kernels[] = {HS_K4(hs_thread_kernel_wide, HS_WF_FAULTS | HS_WF_PROFILE)};
     /* small launches (every block resident at 4 blocks per SM, no shared-memory heap top, not linked): the spill-free
      * instantiation, see hs_thread_kernel_wide */
@@ -500,7 +508,8 @@ static int launch_thread(hs_engine *E, hs_kernel_run R, const hs_kernel_out &O, 
     const hs_launch_info info = {3, wide ? (uint32_t)HS_KERNEL_THREAD_WIDE : (uint32_t)HS_KERNEL_THREAD, (uint32_t)fl,
                                  R.lane_stride, R.heap_top, tblocks, HS_THREAD_BLOCK, (uint32_t)dyn_smem};
     const kernel kern = !(fl & HS_WF_FAULTS) ? (wide ? wide_kernels[fl] : kernels[fl])
-                      : wide ? fault_wide_kernels[fl & 3] : fault_kernels[(fl & 3) | ((fl & HS_WF_HEAPTOP) ? 4 : 0)];
+                      : wide ? fault_wide_kernels[fl & 3]
+                      : fault_kernels[(fl & 3) | ((fl & HS_WF_HEAPTOP) ? 4 : 0) | ((fl & HS_WF_LINKED) ? 8 : 0)];
     return timed_launch(E, info, kern, M, R, (unsigned char *)E->d_state.p, (hs_wring_entry *)E->d_rings.p, O);
 }
 #undef HS_K4
@@ -519,6 +528,8 @@ int hs_last_error(char *buf, int len)
 }
 
 int hs_model_validate(const hs_model_desc *model) { return validate_model(model); }
+
+int hs_partition_validate(const hs_model_desc *model) { return validate_model(model, true); }
 
 int hs_engine_create(int device, void *stream, hs_engine **out)
 {
@@ -560,10 +571,10 @@ int hs_engine_destroy(hs_engine *E)
     return HS_OK;
 }
 
-int hs_model_upload(hs_engine *E, const hs_model_desc *m)
+static int model_upload(hs_engine *E, const hs_model_desc *m, bool partition)
 {
     if (!E) return fail(HS_ERR_INVALID, "engine is NULL");
-    int rc = validate_model(m);
+    int rc = validate_model(m, partition);
     if (rc) return rc;
     CUDA_TRY(cudaSetDevice(E->device));
     uint32_t n = m->n_entities;
@@ -642,9 +653,14 @@ int hs_model_upload(hs_engine *E, const hs_model_desc *m)
     CUDA_TRY(cudaStreamSynchronize(E->stream));   /* host vectors may be reused by the caller's next upload */
     E->lane_ok = classify_lane(E);
     E->have_model = true;
-    E->have_run = keep_run;
+    E->have_run = keep_run && E->partition == partition;
+    E->partition = partition;
     return HS_OK;
 }
+
+int hs_model_upload(hs_engine *E, const hs_model_desc *m) { return model_upload(E, m, false); }
+
+int hs_partition_upload(hs_engine *E, const hs_model_desc *m) { return model_upload(E, m, true); }
 
 
 int hs_run(hs_engine *E, const hs_run_params *p)
@@ -664,7 +680,8 @@ int hs_run(hs_engine *E, const hs_run_params *p)
     if (engine < 1 || engine > 3) return fail(HS_ERR_INVALID, "unknown engine %d", engine);
     if (linked && engine != 3) return fail(HS_ERR_INVALID, "linked partitions run on the thread engine (engine 3)");
     const bool faults = std::any_of(E->ents.begin(), E->ents.end(), [](const hs_entity_desc &e) { return e.kind == HS_ENT_FAULT; });
-    if (faults && linked) return fail(HS_ERR_INVALID, "a linked partition cannot have FAULT rows (fault schedules)");
+    if (faults && linked && !E->partition)
+        return fail(HS_ERR_INVALID, "a linked partition with FAULT rows (a fault schedule) is uploaded with hs_partition_upload");
     if (engine == 2 && faults) return fail(HS_ERR_INVALID, "the lane engine does not run fault schedules (the model has FAULT rows): use engine 0, 1 or 3");
     if (engine == 2 && !E->lane_ok) return fail(HS_ERR_INVALID, "lane engine needs Source -> Server(concurrency <= 64) -> Sink|Counter");
 

@@ -676,7 +676,9 @@ hs_thread_body(const hs_warp_model &M, const hs_kernel_run &P, unsigned char *__
     };
     /* linked partitions: what the coordinator delivered at the last barrier is scheduled before the first pop
      * (WindowedCoordinator._exchange_events -> Simulation.schedule = heap push, core/simulation.py:195-206); an event
-     * that lies behind this replica's clock is dropped by the time-travel test when it is popped */
+     * that lies behind this replica's clock is dropped by the time-travel test when it is popped.  A delivered event keeps
+     * its sender's sort index, so it can tie with a pending FAULT event of this partition: heap_push_key runs the same
+     * fault_tie test as for an in-run push (HS_ST_FAULT_TIE).  FAULT rows are pushed at window 0 only (the bootstrap). */
     if ((FLAGS & HS_WF_LINKED) && M.inbox_cap && O.inbox_n) {
         const uint32_t n_in = O.inbox_n[r];
         for (uint32_t k = 0; k < n_in; ++k) {

@@ -29,7 +29,8 @@ EXPORTED_SYMBOLS = ["hs_version", "hs_last_error", "hs_engine_create", "hs_engin
                     "hs_model_validate", "hs_run", "hs_set_trace", "hs_sync", "hs_last_run_ms", "hs_launch_count",
                     "hs_last_launch", "hs_read_outputs", "hs_read_totals", "hs_read_cell_totals", "hs_totals_device_ptr",
                     "hs_sketch_layout", "hs_read_sketches", "hs_coordinator_create", "hs_coordinator_destroy",
-                    "hs_coordinator_exchange", "hs_coordinator_read", "hs_read_outbox", "hs_read_inbox"]
+                    "hs_coordinator_exchange", "hs_coordinator_read", "hs_read_outbox", "hs_read_inbox",
+                    "hs_partition_upload", "hs_partition_validate"]
 
 
 def load_library(path: str | None = None):
@@ -54,6 +55,8 @@ def load_library(path: str | None = None):
         "hs_engine_destroy": ([H], C.c_int),
         "hs_model_upload": ([H, C.POINTER(A.ModelDesc)], C.c_int),
         "hs_model_validate": ([C.POINTER(A.ModelDesc)], C.c_int),
+        "hs_partition_upload": ([H, C.POINTER(A.ModelDesc)], C.c_int),
+        "hs_partition_validate": ([C.POINTER(A.ModelDesc)], C.c_int),
         "hs_run": ([H, C.POINTER(A.RunParams)], C.c_int),
         "hs_set_trace": ([H, C.POINTER(C.c_double), C.c_uint64, C.POINTER(C.c_double), C.c_uint64, C.c_uint32], C.c_int),
         "hs_sync": ([H], C.c_int),
@@ -90,10 +93,11 @@ def _check(L, rc: int):
         raise EngineError(rc, buf.value.decode(errors="replace"))
 
 
-def validate_model(model: FlatModel) -> None:
+def validate_model(model: FlatModel, partition: bool = False) -> None:
+    """hs_model_validate, or hs_partition_validate for ``partition`` (a partition of a linked run)"""
     L = load_library()
     d = model.desc()
-    _check(L, L.hs_model_validate(C.byref(d)))
+    _check(L, (L.hs_partition_validate if partition else L.hs_model_validate)(C.byref(d)))
 
 
 def make_params(*, seed=1234, end_ns, n_replicas=1, seed_stride=0, rid_base=0, rid_stride=1,
@@ -170,9 +174,10 @@ class Engine:
         except Exception:
             pass
 
-    def upload(self, model: FlatModel) -> None:
+    def upload(self, model: FlatModel, partition: bool = False) -> None:
+        """hs_model_upload, or hs_partition_upload for ``partition`` (a partition of a linked run)"""
         d = model.desc()
-        _check(self._L, self._L.hs_model_upload(self._h, C.byref(d)))
+        _check(self._L, (self._L.hs_partition_upload if partition else self._L.hs_model_upload)(self._h, C.byref(d)))
         self._model = model
 
     def set_trace(self, arrival_targets=None, service_samples=None) -> None:

@@ -108,7 +108,7 @@ class LinkedRun:
         self._stream_ptr = sp
         self.engines = [_engine.Engine(device, stream=sp) for _ in lm.models]
         for e, m in zip(self.engines, lm.models):
-            e.upload(m)
+            e.upload(m, partition=True)
         self.coordinator = None
         self.windows = 0
 

@@ -13,9 +13,10 @@ import numpy as np
 from dataclasses import dataclass, field
 from typing import Any
 
+from . import _abi as A
 from .api import Instant, Simulation
 from .lowering import UnsupportedModelError
-from .results import EntitySummary, SimulationSummary, replica_summary, write_back
+from .results import EntitySummary, SimulationSummary, fault_cancelled, replica_summary, write_back
 
 
 @dataclass
@@ -96,6 +97,10 @@ def _events_bound(rate: float, inbox_cap: int, end_ns: int) -> float:
     return (rate * 4 + 50.0) * (end_ns / 1e9 + 1.0) + 4.0 * max(inbox_cap, 0)
 
 
+# status bits a linked run reports instead of raising: a tie the reference orders by heapq's array layout (a delivered
+# event with another event; any pushed event with a pending fault event), as Simulation.run reports HS_ST_FAULT_TIE
+_TIES = A.HS_ST_LINK_TIE | A.HS_ST_FAULT_TIE
+
 _RINGS = (("sample_cap", "n_sink_samples", "Sink sample"), ("service_cap", "n_service_samples", "service time"),
           ("record_cap", "events_processed", "event record"))
 
@@ -143,10 +148,6 @@ class ParallelSimulation:
         self._simulations: dict[str, Simulation] = {}
         self._linked = None
         if self._links:
-            for p in partitions:
-                if p.fault_schedule is not None:
-                    raise UnsupportedModelError(f"partition {p.name!r}: fault schedules in linked partitions do not run "
-                                                "on the device (independent partitions do)")
             self._init_linked(start_time, end_time, duration, window_size)
             return
         for k, p in enumerate(partitions):
@@ -165,7 +166,7 @@ class ParallelSimulation:
         """parallel/validation.py:19-110 + parallel/simulation.py:84-150: check the declarations, find the events that
         cross partitions (a Server whose downstream lives elsewhere) and lower every partition to a model of its own."""
         from . import _abi as A
-        from .api import Instant
+        from .api import Instant, _start_schedule
         from .linked import LinkedModel, LinkSpec
         from .lowering import _service, lower
         parts = self._partitions
@@ -223,7 +224,12 @@ class ParallelSimulation:
                                          f"'{getattr(t, 'name', t)}' in partition '{names[d]}' without a PartitionLink "
                                          f"('{p.name}' -> '{names[d]}')")       # validation.py:160-200
                     remote[id(t)] = slot_of[k][d]
-            m, objs = lower(p.sources or [], ents, probes=p.probes or None, horizon_s=self._end_ns / 1e9, remote=remote)
+            if p.fault_schedule is not None:
+                # the partition's own Simulation bootstraps its schedule (parallel/simulation.py:94-104): names resolve
+                # among its objects only, sort indices follow its own sources and probes
+                _start_schedule(p.fault_schedule, p.sources, ents, p.probes)
+            m, objs = lower(p.sources or [], ents, probes=p.probes or None, horizon_s=self._end_ns / 1e9, remote=remote,
+                            fault_schedule=p.fault_schedule)
             models.append(m)
             objects.append(objs)
         for k, m in enumerate(models):      # REMOTE rows: the entity's id over there
@@ -250,7 +256,10 @@ class ParallelSimulation:
         from . import _abi as A
         from .api import Instant
         from .linked import LinkedRun
+        from .lowering import refresh_fault_cancellation
         lm = self._linked
+        for m in lm.models:                 # FaultHandle.cancel() may have been called since the partitions were lowered
+            refresh_fault_cancellation(m)
         t0 = _time.monotonic()
         run = LinkedRun(lm, device=self._device)
         try:
@@ -277,8 +286,8 @@ class ParallelSimulation:
                 status = 0
                 for o in outs:
                     status |= int(np.bitwise_or.reduce(o["summaries"]["status"])) if len(o["summaries"]) else 0
-                clean = not (status & ~A.HS_ST_LINK_TIE) and not over.any()
-                queue_full = bool(status & A.HS_ST_QUEUE_OVERFLOW and not (status & ~(A.HS_ST_QUEUE_OVERFLOW | A.HS_ST_LINK_TIE))
+                clean = not (status & ~_TIES) and not over.any()
+                queue_full = bool(status & A.HS_ST_QUEUE_OVERFLOW and not (status & ~(A.HS_ST_QUEUE_OVERFLOW | _TIES))
                                   and not over.any())
                 short = _short_rings(outs, caps) if clean else []     # counts of a run that stopped early mean nothing
                 if not (queue_full or short):
@@ -293,7 +302,7 @@ class ParallelSimulation:
                                f"{caps[q][cap]} device slots ({cap}) in the last of {attempt + 1} attempts; the ring "
                                "wrapped, so its results are not published")
         wall = _time.monotonic() - t0
-        bad = [(lm.names[q], int(s)) for q, o in enumerate(outs) for s in o["summaries"]["status"] if int(s) & ~A.HS_ST_LINK_TIE]
+        bad = [(lm.names[q], int(s)) for q, o in enumerate(outs) for s in o["summaries"]["status"] if int(s) & ~_TIES]
         if bad or over.any():
             bits = 0
             for _, s_ in bad:
@@ -303,11 +312,12 @@ class ParallelSimulation:
                 why.append(f"a server queue outgrew {ring} device slots (ParallelSimulation.queue_ring)")
             if (bits & A.HS_ST_LINK_OVERFLOW) or over.any():
                 why.append(f"an outbox / inbox outgrew ParallelSimulation.link_buffer = {self.link_buffer}")
-            if bits & ~(A.HS_ST_QUEUE_OVERFLOW | A.HS_ST_LINK_OVERFLOW):
-                why.append(f"status bits {bits & ~(A.HS_ST_QUEUE_OVERFLOW | A.HS_ST_LINK_OVERFLOW):#x}")
+            if bits & ~(A.HS_ST_QUEUE_OVERFLOW | A.HS_ST_LINK_OVERFLOW | _TIES):
+                why.append(f"status bits {bits & ~(A.HS_ST_QUEUE_OVERFLOW | A.HS_ST_LINK_OVERFLOW | _TIES):#x}")
             raise RuntimeError(f"linked run did not complete cleanly: partition status {bad[:4]}, inbox overflows {int(over.sum())}: "
                                + "; ".join(why))
         self.link_ties = int(sum(int(s) & A.HS_ST_LINK_TIE != 0 for o in outs for s in o["summaries"]["status"]))
+        self.fault_ties = int(sum(int(s) & A.HS_ST_FAULT_TIE != 0 for o in outs for s in o["summaries"]["status"]))
         self.last_outputs, self.last_delivered, self.last_lost = outs, delivered, lost
         return outs, delivered, lost, wall, run.windows
 
@@ -324,7 +334,8 @@ class ParallelSimulation:
         for q, name in enumerate(lm.names):
             write_back(lm.models[q], lm.objects[q], outs[q], 0, Instant)
             entities = [o for o in self._partitions[q].entities if any(o is x for x in lm.objects[q])]
-            summaries[name] = replica_summary(outs[q]["summaries"][0], wall, entities)
+            summaries[name] = replica_summary(outs[q]["summaries"][0], wall, entities,
+                                              events_cancelled=fault_cancelled(lm.models[q], outs[q]["entity_stats"][0]))
         n = len(summaries)
         return ParallelSimulationSummary(
             **_aggregate(summaries), wall_clock_seconds=wall,

@@ -70,13 +70,15 @@ enum {
                             aimed at a CallbackEntity that sets (crash, pause) or clears (restart, resume) `_crashed` on
                             the entity it names.  target = that entity, l0 = the event's time in ns (Instant.from_seconds),
                             i1 = 1 set / 0 clear, i2 = 1 if its FaultHandle was cancelled before the run, i3 = its
-                            bootstrap sort index (global counter: sources, then probes, then the faults in schedule order).
+                            bootstrap sort index (global counter: sources, then probes, then the faults in schedule order;
+                            in a linked partition the counter of that partition's own Simulation).
                             While an entity's flag is set, Event.invoke (core/event.py:261-262) drops the events aimed at it
                             -- counted and clock-moving, but neither handler nor completion hooks run: SOURCE_TICK (the
                             source is silent from then on), REQ_ENQUEUE, REQ_SINK, REQ_COUNTER, REQ_SKETCH, REQ_LB,
                             LB_RESPONSE.  hs_entity_stats: c0 = fired, c1 = popped while cancelled (events_cancelled,
-                            core/simulation.py:475-477: not processed, the clock does not move).  Not in models with
-                            REMOTE rows; the lane engine does not run them                                  */
+                            core/simulation.py:475-477: not processed, the clock does not move).  A fault cannot target a
+                            REMOTE row, and it sits next to REMOTE rows only in a model uploaded with
+                            hs_partition_upload; the lane engine does not run them                          */
     HS_ENT_REMOTE = 9    /* stand-in for an entity that lives in ANOTHER partition of a ParallelSimulation
                             (parallel/simulation.py:31, parallel/routing.py:17-63): an event whose target is this row
                             is never scheduled here -- the partition's router puts it, with its send time, into the
@@ -254,8 +256,9 @@ typedef struct hs_run_params {
                                      and sort index (the indices come from different partitions' counters).  The reference
                                      orders such a pair by the accident of heapq's array layout; the engines order it by
                                      their own heap's, so this replica's event order may differ from the reference's      */
-#define HS_ST_FAULT_TIE 256u      /* an event created during the run tied with a pending FAULT event on both time and sort
-                                     index (the fault's index comes from the bootstrap counter, the other's from the run's):
+#define HS_ST_FAULT_TIE 256u      /* an event created during the run, or delivered over a link, tied with a pending FAULT
+                                     event on both time and sort index (the fault's index comes from the bootstrap counter,
+                                     the other's from the run's or from the sending partition's):
                                      heapq orders such a pair by its array layout, the engines by their own heap's, so this
                                      replica's event order may differ from the reference's                               */
 
@@ -358,6 +361,13 @@ int hs_model_upload(hs_engine *e, const hs_model_desc *model);
 
 /* Validate a model without a device (used by host-side tests). */
 int hs_model_validate(const hs_model_desc *model);
+
+/* hs_model_upload / hs_model_validate for one partition of a linked run (ParallelSimulation with PartitionLinks,
+ * parallel/simulation.py:94-104): the partition's Simulation bootstraps its own fault schedule, so FAULT rows may sit
+ * next to its REMOTE rows (a FAULT row still cannot target one).  A model uploaded with hs_model_upload that has
+ * FAULT rows does not run as a linked partition (hs_run with outbox / inbox / HS_RUN_LINKED). */
+int hs_partition_upload(hs_engine *e, const hs_model_desc *model);
+int hs_partition_validate(const hs_model_desc *model);
 
 /* Byte offsets of the SKETCH rows' state.  per_replica[i] / merged[i] = offset of entity i's state in
  * one replica's slice of hs_outputs.sketches / in the merged image (0 for other kinds); a replica's
