@@ -3,7 +3,7 @@ from __future__ import annotations
 
 import ctypes as C
 
-HS_ABI_VERSION = 6
+HS_ABI_VERSION = 7
 
 HS_OK, HS_ERR_INVALID, HS_ERR_CUDA, HS_ERR_NO_DEVICE, HS_ERR_STATE, HS_ERR_OVERFLOW = 0, -1, -2, -3, -4, -5
 
@@ -150,6 +150,11 @@ ENTITY_DTYPE = _np.dtype([("kind", "<i4"), ("target", "<i4"), ("i0", "<i4"), ("i
                           ("i3", "<i4"), ("l0", "<i8"), ("d0", "<f8"), ("d1", "<f8")])
 assert SUMMARY_DTYPE.itemsize == 56 and STATS_DTYPE.itemsize == 64 and RECORD_DTYPE.itemsize == 16
 assert ENTITY_DTYPE.itemsize == 48
+# time buckets (hs_set_buckets): hs_bucket, 32 bytes, and hs_bucket_total, 48 bytes
+BUCKET_DTYPE = _np.dtype([("count", "<i8"), ("sum", "<f8"), ("comp", "<f8"), ("max", "<f8")])
+BUCKET_TOTAL_DTYPE = _np.dtype([("replicas", "<i8"), ("count", "<i8"), ("sum", "<f8"), ("mean_sum", "<f8"),
+                                ("mean_sq_sum", "<f8"), ("max", "<f8")])
+assert BUCKET_DTYPE.itemsize == 32 and BUCKET_TOTAL_DTYPE.itemsize == 48
 PROFILE_DTYPE = _np.dtype([("kind", "<i4"), ("pad", "<i4"), ("p", "<f8", (4,))])
 assert PROFILE_DTYPE.itemsize == 40
 

@@ -22,6 +22,7 @@ from typing import Any, Callable
 import numpy as np
 
 from . import _abi as A
+from . import buckets as _buckets
 from . import lowering
 from .engine import Engine, make_params
 from .results import EntitySummary, QueueStats, SimulationSummary, fault_cancelled, replica_summary, write_back  # noqa: F401
@@ -798,7 +799,7 @@ class Simulation:
     def run_ensemble(self, n_replicas: int, *, seed: int | None = None, seed_stride: int = 0, rid_base: int = 0,
                      rid_stride: int = 1, replica_index_base: int = 0, replicas_per_cell: int = 1,
                      window_end_s: float | None = None, resume: bool = False, host: dict | None = None,
-                     upload: bool = True, totals: bool = True, on_overflow: str = "grow", **caps):
+                     upload: bool = True, totals: bool = True, on_overflow: str = "grow", buckets=None, **caps):
         """N independent replicas of this model on the device; returns the raw per-replica arrays
         (summaries, entity_stats, optional recorder rings) and the engine's totals.
 
@@ -808,7 +809,19 @@ class Simulation:
 
         Every replica's ``status`` is checked.  A device queue ring that overflowed (the reference's queues are
         unbounded) is handled per ``on_overflow``: "grow" re-runs the ensemble with doubled rings (fresh,
-        unwindowed runs only), "raise" raises, "ignore" returns the flagged statuses to the caller."""
+        unwindowed runs only), "raise" raises, "ignore" returns the flagged statuses to the caller.
+
+        ``buckets=(width_s, n)`` reduces every replica's Sink / LatencyTracker / ThroughputTracker / Probe samples into
+        ``Data.bucket(width_s)`` on the device (n buckets per row; n * width_s must exceed the end time) and adds
+        ``out["buckets"]`` (BUCKET_DTYPE [replica, row, n + 1]; slot n holds the samples of the event processed past the
+        end time, whose index is ``out["bucket_past_end"][replica, row]``), ``out["bucket_totals"]`` (BUCKET_TOTAL_DTYPE
+        [cell, row, n + 1], cells as ``replicas_per_cell`` and the model's sweep cells define them, one for a plain
+        ensemble), ``out["bucket_rows"]`` (entity ids) and ``out["bucket_objects"]`` (the object of each row).
+        ``buckets.bucketed_data(out, obj, replica)`` gives one replica's ``BucketedData``.  A bucketed run has no
+        recorder rings; every window of a windowed run passes the same ``buckets``, and only the window that reaches the
+        end time reads them back (the records are gigabytes at full size; ``Engine.read_buckets`` reads them after any
+        window)."""
+        spec = _buckets.check_spec(buckets, self._end_time.nanoseconds) if buckets is not None else None
         eng = _engine(self._device)
         if lowering.refresh_fault_cancellation(self.model) and not upload and not resume:
             upload = True                   # a FaultHandle was cancelled since the last upload
@@ -822,6 +835,29 @@ class Simulation:
             w = int(round(float(window_end_s) * 1e9))
             we = w if w < end_ns else -1
         ring = int(caps.pop("queue_ring", 0) or 0)
+        eng.set_buckets(*(spec or (0.0, 0)))
+        try:
+            out, st, ring = self._run_windows(eng, n_replicas, seed, seed_stride, rid_base, rid_stride, replica_index_base,
+                                              replicas_per_cell, end_ns, we, resume, ring, host, on_overflow, caps)
+            if spec and we < 0:
+                w, nb = spec
+                out["buckets"], out["bucket_past_end"] = eng.read_buckets(nb)
+                n_cells = max(1, int(self.model.n_cells))
+                out["bucket_totals"] = eng.read_bucket_totals(n_cells, out["buckets"].shape[1], nb)
+                out["bucket_width_s"], out["bucket_count"] = w, nb
+                out["bucket_rows"] = _buckets.rows(self.model)
+                out["bucket_objects"] = _buckets.row_objects(self.model, self.objects)
+        finally:
+            eng.set_buckets(0.0, 0)             # the engine is shared: other runs get no buckets unless they ask
+        out["status"] = st
+        out["queue_ring"] = ring
+        if totals:
+            out["totals"] = eng.read_totals()
+        out["device_ms"] = eng.last_run_ms()
+        return out
+
+    def _run_windows(self, eng, n_replicas, seed, seed_stride, rid_base, rid_stride, replica_index_base, replicas_per_cell,
+                     end_ns, we, resume, ring, host, on_overflow, caps):
         bad = A.HS_ST_QUEUE_OVERFLOW | A.HS_ST_FEL_OVERFLOW | A.HS_ST_SKETCH_OVERFLOW
         for _ in range(12):
             eng.run(make_params(seed=self._seed if seed is None else seed, seed_stride=seed_stride, rid_base=rid_base,
@@ -842,12 +878,7 @@ class Simulation:
                                       f"full); pass a larger queue_ring=", st.copy())
         if "max_events" in caps and int((st & A.HS_ST_EVENT_LIMIT != 0).sum()) and on_overflow != "ignore":
             raise EnsembleStatusError("max_events reached before end_time", st.copy())
-        out["status"] = st
-        out["queue_ring"] = ring
-        if totals:
-            out["totals"] = eng.read_totals()
-        out["device_ms"] = eng.last_run_ms()
-        return out
+        return out, st, ring
 
 
 class EnsembleStatusError(RuntimeError):
@@ -1073,7 +1104,8 @@ class ParallelRunner:
 
     def run_replicas(self, build_fn: Callable, n_replicas: int, base_seed: int = 42, **caps):
         """Returns a list-like of ParallelResult (materialised on access).  Device queue rings that overflow
-        are grown and the ensemble re-run (``Simulation.run_ensemble``); every result carries ``status``."""
+        are grown and the ensemble re-run (``Simulation.run_ensemble``); every result carries ``status``.
+        ``buckets=(width_s, n)`` goes to ``run_ensemble``: the time buckets are in the returned list's ``.raw``."""
         sim = build_fn()
         t0 = _time.monotonic()
         out = sim.run_ensemble(n_replicas, seed=base_seed, seed_stride=1, rid_base=sim._replica, rid_stride=0,

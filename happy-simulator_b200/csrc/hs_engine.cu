@@ -97,6 +97,11 @@ struct hs_engine {
     dev_buf d_outbox, d_outbox_n, d_inbox, d_inbox_n;
     uint32_t link_replicas = 0;                 /* replicas the outbox / inbox buffers are sized for */
     bool partition = false;                     /* the model came through hs_partition_upload */
+    /* time buckets (hs_set_buckets): the configuration for the next runs, the last run's, the model's bucketed rows */
+    double bkt_w = 0.0; uint32_t bkt_n = 0;
+    double last_bkt_w = 0.0; uint32_t last_bkt_n = 0;
+    uint32_t bkt_rows = 0;
+    dev_buf d_buckets, d_bkt_past, d_bkt_partial, d_bkt_out, d_bkt_index;
 };
 
 /* ---- validation ----------------------------------------------------------- */
@@ -347,7 +352,8 @@ static int timed_launch(hs_engine *E, const hs_launch_info &info, Kernel kern, A
 
 #define HS_K4(K, F) K<F>, K<F + 1>, K<F + 2>, K<F + 3>
 
-static int launch_lane(hs_engine *E, const hs_kernel_run &R, const hs_kernel_out &O, bool want_hash, bool want_rec)
+static int launch_lane(hs_engine *E, const hs_kernel_run &R, const hs_kernel_out &O, bool want_hash, bool want_rec,
+                       const hs_bucket_args &BK)
 {
     const hs_lane_model &M = E->lane_model;
     const uint32_t n = R.n_replicas;
@@ -358,23 +364,33 @@ static int launch_lane(hs_engine *E, const hs_kernel_run &R, const hs_kernel_out
     const bool simple = !M.has_profile && !R.trace_arr && !R.trace_svc && M.arr_kind == HS_ARR_POISSON &&
                         M.svc_kind == HS_SVC_EXPONENTIAL && M.policy == HS_Q_FIFO && M.capacity < 0 &&
                         M.stop_after < 0 && M.dst_id >= 0 && M.dst_kind == HS_ENT_SINK && M.c_max == 1;
+    const bool buckets = BK.n != 0;                /* never with the recorder: hs_run refuses that combination */
     const int fl = (want_hash ? HS_LF_HASH : 0) | (want_rec ? HS_LF_REC : 0) |
-                   (M.has_profile ? HS_LF_PROFILE : 0) | (simple ? HS_LF_SIMPLE : 0);
-    using kernel = void (*)(hs_lane_model, hs_kernel_run, hs_lane_state *, hs_ring_entry *, hs_cont *, hs_kernel_out);
+                   (M.has_profile ? HS_LF_PROFILE : 0) | (simple ? HS_LF_SIMPLE : 0) | (buckets ? HS_LF_BUCKETS : 0);
+    using kernel = void (*)(hs_lane_model, hs_kernel_run, hs_lane_state *, hs_ring_entry *, hs_cont *, hs_kernel_out, hs_no_bucket_args);
+    using bucket_kernel = void (*)(hs_lane_model, hs_kernel_run, hs_lane_state *, hs_ring_entry *, hs_cont *, hs_kernel_out, hs_bucket_args);
     static const kernel kernels[] = {HS_K4(hs_lane_kernel, 0), HS_K4(hs_lane_kernel, 4),     /* fl <= 11: the SIMPLE */
                                      HS_K4(hs_lane_kernel, 8)};                               /* model has no profile */
+    /* [HASH | PROFILE ? 2 : 0 | SIMPLE ? 4 : 0] */
+    static const bucket_kernel bucket_kernels[] = {hs_lane_kernel<HS_LF_BUCKETS>, hs_lane_kernel<HS_LF_BUCKETS | HS_LF_HASH>,
+                                            hs_lane_kernel<HS_LF_BUCKETS | HS_LF_PROFILE>, hs_lane_kernel<HS_LF_BUCKETS | HS_LF_PROFILE | HS_LF_HASH>,
+                                            hs_lane_kernel<HS_LF_BUCKETS | HS_LF_SIMPLE>, hs_lane_kernel<HS_LF_BUCKETS | HS_LF_SIMPLE | HS_LF_HASH>};
     const hs_launch_info info = {2, HS_KERNEL_LANE, (uint32_t)fl, 1, 0, (n + HS_LANE_THREADS - 1) / HS_LANE_THREADS,
                                  HS_LANE_THREADS, 0};
+    if (buckets)
+        return timed_launch(E, info, bucket_kernels[(fl & HS_LF_HASH) | (M.has_profile ? 2 : 0) | (simple ? 4 : 0)], M, R,
+                            (hs_lane_state *)E->d_state.p, (hs_ring_entry *)E->d_rings.p, (hs_cont *)E->d_conts.p, O, BK);
     return timed_launch(E, info, kernels[fl], M, R, (hs_lane_state *)E->d_state.p, (hs_ring_entry *)E->d_rings.p,
-                        (hs_cont *)E->d_conts.p, O);
+                        (hs_cont *)E->d_conts.p, O, hs_no_bucket_args());
 }
 
 static const uint32_t HS_WARP_SMEM_MAX = 227 * 1024 - 1024;      /* dynamic shared memory of a warp-engine CTA */
 
 /* What the warp and the thread engine share: the future-event slots, the servers' queue-ring indices, the replica
- * state and queue-ring buffers, and the model flags (*fl). */
+ * state and queue-ring buffers, and the model flags (*fl).  A bucketed run (BK->n != 0) appends the rows' time-bucket
+ * accumulators to the replica block and sets BK->acc_off to their offset. */
 static int general_setup(hs_engine *E, const hs_kernel_run &R, bool thread, bool want_hash, bool want_rec,
-                         hs_warp_model &M, int *fl)
+                         hs_warp_model &M, int *fl, hs_bucket_args *BK)
 {
     const uint32_t n = R.n_replicas;
     const uint32_t ne = (uint32_t)E->ents.size();
@@ -397,10 +413,15 @@ static int general_setup(hs_engine *E, const hs_kernel_run &R, bool thread, bool
     const uint32_t S = (uint32_t)((live + 31) / 32) * 32;
     if (S > 65535) return fail(HS_ERR_INVALID, "model needs %u future-event slots (limit 65535)", S);
     /* thread engine: 4-ary key heap + payload slots instead of the warp engine's SoA slot table */
-    const uint32_t block_bytes = thread
+    uint32_t block_bytes = thread
         ? hs_thread_offsets(ne, S).total
         : (uint32_t)(sizeof(hs_warp_hdr) + (size_t)ne * sizeof(hs_went) + (((size_t)S * 46 + 15) / 16) * 16 +
                      (size_t)HS_W_NCAP * sizeof(hs_wnow));
+    if (BK->n) {                                     /* whole lines (thread engine) / 16-byte units (TMA) */
+        const uint32_t unit = thread ? 128u : 16u;
+        BK->acc_off = block_bytes;
+        block_bytes += (uint32_t)((BK->rows * sizeof(hs_bucket_acc) + unit - 1) / unit * unit);
+    }
     /* the warp engine stages a replica's block (and an mbarrier slot) in shared memory */
     if (!thread && 16 + block_bytes > HS_WARP_SMEM_MAX)
         return fail(HS_ERR_INVALID, "model too large for the warp engine (%u B of state per replica)", 16 + block_bytes);
@@ -431,11 +452,12 @@ static int general_setup(hs_engine *E, const hs_kernel_run &R, bool thread, bool
     return HS_OK;
 }
 
-static int launch_warp(hs_engine *E, const hs_kernel_run &R, const hs_kernel_out &O, bool want_hash, bool want_rec)
+static int launch_warp(hs_engine *E, const hs_kernel_run &R, const hs_kernel_out &O, bool want_hash, bool want_rec,
+                       hs_bucket_args BK)
 {
     hs_warp_model M;
     int fl, rc;
-    if ((rc = general_setup(E, R, false, want_hash, want_rec, M, &fl))) return rc;
+    if ((rc = general_setup(E, R, false, want_hash, want_rec, M, &fl, &BK))) return rc;
     /* per warp its replica's block behind an mbarrier slot; per CTA a copy of the model tables when they fit */
     const uint32_t ne = M.n_entities;
     const uint32_t per_warp = 16 + M.block_bytes;
@@ -450,21 +472,33 @@ static int launch_warp(hs_engine *E, const hs_kernel_run &R, const hs_kernel_out
     const uint32_t grid = std::min<uint32_t>((R.n_replicas + warps - 1) / warps, (uint32_t)E->sm_count * blocks_per_sm);
     if ((rc = E->d_counter.ensure(16))) return rc;
     CUDA_TRY(cudaMemsetAsync(E->d_counter.p, 0, 16, E->stream));
-    using kernel = void (*)(hs_warp_model, hs_kernel_run, unsigned char *, hs_wring_entry *, hs_kernel_out, unsigned int *);
+    using kernel = void (*)(hs_warp_model, hs_kernel_run, unsigned char *, hs_wring_entry *, hs_kernel_out, unsigned int *, hs_no_bucket_args);
+    using bucket_kernel = void (*)(hs_warp_model, hs_kernel_run, unsigned char *, hs_wring_entry *, hs_kernel_out, unsigned int *, hs_bucket_args);
     static const kernel kernels[] = {HS_K4(hs_warp_kernel, 0), HS_K4(hs_warp_kernel, 4)};
     static const kernel fault_kernels[] = {HS_K4(hs_warp_kernel, HS_WF_FAULTS | HS_WF_PROFILE)};
+    /* time buckets (never with the recorder): [HASH | FAULTS ? 2 : 0], the profile path always compiled in */
+    static const bucket_kernel bucket_kernels[] = {hs_warp_kernel<HS_WF_BUCKETS | HS_WF_PROFILE>, hs_warp_kernel<HS_WF_BUCKETS | HS_WF_PROFILE | HS_WF_HASH>,
+                                            hs_warp_kernel<HS_WF_BUCKETS | HS_WF_FAULTS | HS_WF_PROFILE>,
+                                            hs_warp_kernel<HS_WF_BUCKETS | HS_WF_FAULTS | HS_WF_PROFILE | HS_WF_HASH>};
+    const hs_launch_info info = {1, HS_KERNEL_WARP, (uint32_t)(fl | (BK.n ? HS_WF_BUCKETS | HS_WF_PROFILE : 0)), 1, 0, grid, warps * 32, smem};
+    if (BK.n) {
+        const bucket_kernel kern = bucket_kernels[(fl & HS_WF_HASH) | ((fl & HS_WF_FAULTS) ? 2 : 0)];
+        CUDA_TRY(cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
+        return timed_launch(E, info, kern, M, R, (unsigned char *)E->d_state.p, (hs_wring_entry *)E->d_rings.p, O,
+                            (unsigned int *)E->d_counter.p, BK);
+    }
     const kernel kern = (fl & HS_WF_FAULTS) ? fault_kernels[fl & 3] : kernels[fl];
     CUDA_TRY(cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
-    const hs_launch_info info = {1, HS_KERNEL_WARP, (uint32_t)fl, 1, 0, grid, warps * 32, smem};
     return timed_launch(E, info, kern, M, R, (unsigned char *)E->d_state.p,
-                        (hs_wring_entry *)E->d_rings.p, O, (unsigned int *)E->d_counter.p);
+                        (hs_wring_entry *)E->d_rings.p, O, (unsigned int *)E->d_counter.p, hs_no_bucket_args());
 }
 
-static int launch_thread(hs_engine *E, hs_kernel_run R, const hs_kernel_out &O, bool want_hash, bool want_rec, bool linked)
+static int launch_thread(hs_engine *E, hs_kernel_run R, const hs_kernel_out &O, bool want_hash, bool want_rec, bool linked,
+                         hs_bucket_args BK)
 {
     hs_warp_model M;
     int fl, rc;
-    if ((rc = general_setup(E, R, true, want_hash, want_rec, M, &fl))) return rc;
+    if ((rc = general_setup(E, R, true, want_hash, want_rec, M, &fl, &BK))) return rc;
     const uint32_t n = R.n_replicas, ne = M.n_entities, S = M.fel_slots;
     /* entity-owned payload slots: every entity has at most one pending future event; delivered events need slots of their own */
     bool fixed = ne <= S && E->inbox_cap == 0;
@@ -491,6 +525,7 @@ static int launch_thread(hs_engine *E, hs_kernel_run R, const hs_kernel_out &O, 
     R.heap_top = (top < 1 + HS_T_ARITY || R.lane_stride == 32) ? 0 : top;  /* one replica per warp: its heap sits in L1 anyway */
     const size_t dyn_smem = (size_t)(HS_T_KS * 3u + R.heap_top) * rpb * 16;
     using kernel = void (*)(hs_warp_model, hs_kernel_run, unsigned char *, hs_wring_entry *, hs_kernel_out);
+    using bucket_kernel = void (*)(hs_warp_model, hs_kernel_run, unsigned char *, hs_wring_entry *, hs_kernel_out, hs_bucket_args);
     static const kernel kernels[] = {HS_K4(hs_thread_kernel, 0), HS_K4(hs_thread_kernel, 4), HS_K4(hs_thread_kernel, 8),
                                      HS_K4(hs_thread_kernel, 12), HS_K4(hs_thread_kernel, 16), HS_K4(hs_thread_kernel, 20),
                                      HS_K4(hs_thread_kernel, 24), HS_K4(hs_thread_kernel, 28)};
@@ -501,12 +536,28 @@ static int launch_thread(hs_engine *E, hs_kernel_run R, const hs_kernel_out &O, 
                                            HS_K4(hs_thread_kernel, HS_WF_LINKED | HS_WF_FAULTS | HS_WF_PROFILE),
                                            HS_K4(hs_thread_kernel, HS_WF_LINKED | HS_WF_FAULTS | HS_WF_HEAPTOP | HS_WF_PROFILE)};
     static const kernel fault_wide_kernels[] = {HS_K4(hs_thread_kernel_wide, HS_WF_FAULTS | HS_WF_PROFILE)};
+    /* time buckets (never with the recorder, never linked), the profile path always compiled in:
+     * [HASH | HEAPTOP ? 2 : 0 | FAULTS ? 4 : 0] and, wide, [HASH | FAULTS ? 2 : 0] */
+#define HS_TB_(F) hs_thread_bucket_kernel<HS_WF_BUCKETS | HS_WF_PROFILE | (F)>
+    static const bucket_kernel bucket_kernels[] = {HS_TB_(0), HS_TB_(HS_WF_HASH), HS_TB_(HS_WF_HEAPTOP), HS_TB_(HS_WF_HEAPTOP | HS_WF_HASH),
+                                            HS_TB_(HS_WF_FAULTS), HS_TB_(HS_WF_FAULTS | HS_WF_HASH),
+                                            HS_TB_(HS_WF_FAULTS | HS_WF_HEAPTOP), HS_TB_(HS_WF_FAULTS | HS_WF_HEAPTOP | HS_WF_HASH)};
+#undef HS_TB_
+#define HS_TBW_(F) hs_thread_bucket_kernel_wide<HS_WF_BUCKETS | HS_WF_PROFILE | (F)>
+    static const bucket_kernel bucket_wide_kernels[] = {HS_TBW_(0), HS_TBW_(HS_WF_HASH), HS_TBW_(HS_WF_FAULTS), HS_TBW_(HS_WF_FAULTS | HS_WF_HASH)};
+#undef HS_TBW_
+    if (BK.n) fl |= HS_WF_BUCKETS | HS_WF_PROFILE;
     /* small launches (every block resident at 4 blocks per SM, no shared-memory heap top, not linked): the spill-free
      * instantiation, see hs_thread_kernel_wide */
     const bool wide = !R.heap_top && !linked && tblocks <= (uint32_t)E->sm_count * HS_T_WIDE_BLOCKS;
     if (!wide) fl |= (R.heap_top ? HS_WF_HEAPTOP : 0) | (linked ? HS_WF_LINKED : 0);
     const hs_launch_info info = {3, wide ? (uint32_t)HS_KERNEL_THREAD_WIDE : (uint32_t)HS_KERNEL_THREAD, (uint32_t)fl,
                                  R.lane_stride, R.heap_top, tblocks, HS_THREAD_BLOCK, (uint32_t)dyn_smem};
+    if (fl & HS_WF_BUCKETS) {
+        const bucket_kernel kern = wide ? bucket_wide_kernels[(fl & HS_WF_HASH) | ((fl & HS_WF_FAULTS) ? 2 : 0)]
+                                        : bucket_kernels[(fl & HS_WF_HASH) | ((fl & HS_WF_HEAPTOP) ? 2 : 0) | ((fl & HS_WF_FAULTS) ? 4 : 0)];
+        return timed_launch(E, info, kern, M, R, (unsigned char *)E->d_state.p, (hs_wring_entry *)E->d_rings.p, O, BK);
+    }
     const kernel kern = !(fl & HS_WF_FAULTS) ? (wide ? wide_kernels[fl] : kernels[fl])
                       : wide ? fault_wide_kernels[fl & 3]
                       : fault_kernels[(fl & 3) | ((fl & HS_WF_HEAPTOP) ? 4 : 0) | ((fl & HS_WF_LINKED) ? 8 : 0)];
@@ -562,7 +613,8 @@ int hs_engine_destroy(hs_engine *E)
                        &E->d_rings, &E->d_summ, &E->d_stats, &E->d_rec, &E->d_smp, &E->d_svc, &E->d_partials, &E->d_totals,
                        &E->d_srv_index, &E->d_counter, &E->d_trace_arr, &E->d_trace_svc, &E->d_profiles, &E->d_profile_table, &E->d_hist, &E->d_cell_totals, &E->d_conts,
                        &E->d_sketch_tab, &E->d_sketch, &E->d_sketch_merged, &E->d_key_cdf,
-                       &E->d_outbox, &E->d_outbox_n, &E->d_inbox, &E->d_inbox_n};
+                       &E->d_outbox, &E->d_outbox_n, &E->d_inbox, &E->d_inbox_n,
+                       &E->d_buckets, &E->d_bkt_past, &E->d_bkt_partial, &E->d_bkt_out, &E->d_bkt_index};
     for (dev_buf *b : bufs) b->release();
     if (E->ev0) cudaEventDestroy(E->ev0);
     if (E->ev1) cudaEventDestroy(E->ev1);
@@ -624,14 +676,16 @@ static int model_upload(hs_engine *E, const hs_model_desc *m, bool partition)
     /* device copy of the entity rows: the reserved d1 carries the server's index among the servers
      * (= its queue ring) or the SKETCH row's state offset, so the kernels get it with the row */
     std::vector<hs_entity_desc> dev_ents(E->ents);
+    uint32_t rows = 0;
     {
         int64_t k = 0;
         for (uint32_t i = 0; i < n; ++i) {
             hs_entity_desc &e = dev_ents[i];
             /* SERVER: its index among the queue rings; SKETCH: the offset of its state; CACHE_SERVER: both,
-             * ring index in the low 24 bits, state offset above */
+             * ring index in the low 24 bits, state offset above; SINK, PROBE: its bucketed row (hs_set_buckets) */
             const int64_t v = (e.kind == HS_ENT_SERVER) ? k++ : (e.kind == HS_ENT_SKETCH) ? (int64_t)E->sk_off[i]
-                            : (e.kind == HS_ENT_CACHE_SERVER) ? ((k++) | ((int64_t)E->sk_off[i] << 24)) : -1;
+                            : (e.kind == HS_ENT_CACHE_SERVER) ? ((k++) | ((int64_t)E->sk_off[i] << 24))
+                            : (e.kind == HS_ENT_SINK || e.kind == HS_ENT_PROBE) ? (int64_t)rows++ : -1;
             memcpy(&e.d1, &v, 8);
         }
     }
@@ -651,6 +705,7 @@ static int model_upload(hs_engine *E, const hs_model_desc *m, bool partition)
         }
     if ((rc = up(E->d_profiles, E->profiles.data(), E->profiles.size() * sizeof(hs_profile_desc)))) return rc;
     CUDA_TRY(cudaStreamSynchronize(E->stream));   /* host vectors may be reused by the caller's next upload */
+    E->bkt_rows = rows;
     E->lane_ok = classify_lane(E);
     E->have_model = true;
     E->have_run = keep_run && E->partition == partition;
@@ -697,12 +752,39 @@ int hs_run(hs_engine *E, const hs_run_params *p)
             engine != E->last_engine)
             return fail(HS_ERR_STATE, "resume must repeat the replica set, seeds and capacities of the paused run");
         if (want_hist != E->hist_on) return fail(HS_ERR_STATE, "resume must keep HS_RUN_HISTOGRAM");
+        if (E->bkt_n != E->last_bkt_n || (E->bkt_n && E->bkt_w != E->last_bkt_w))
+            return fail(HS_ERR_STATE, "resume must keep the bucket configuration of the paused run (hs_set_buckets)");
         if (ring != E->last_ring) return fail(HS_ERR_STATE, "resume must keep queue_ring");
     }
 
     const uint32_t n = p->n_replicas;
     const uint32_t ne = (uint32_t)E->ents.size();
+    const size_t bkt_records = E->bkt_n ? (size_t)n * E->bkt_rows * ((size_t)E->bkt_n + 1) : 0;
+    if (E->bkt_n) {
+        if (linked) return fail(HS_ERR_INVALID, "time buckets are not available on the windows of a linked partition");
+        if (p->record_cap || p->sample_cap || p->service_cap)
+            return fail(HS_ERR_INVALID, "time buckets are a summary-mode output: run them without recorder rings (record_cap, sample_cap, service_cap = 0)");
+        /* every sample up to end_ns must fall before bucket n: then only the one event processed past end_ns can reach it */
+        const double last = floor(hs_ns_to_seconds(p->end_ns) / E->bkt_w);
+        if (!(last < (double)E->bkt_n))
+            return fail(HS_ERR_INVALID, "%u buckets of %g s end before the end time %.9f s (bucket %.0f): n * width must exceed it",
+                        E->bkt_n, E->bkt_w, hs_ns_to_seconds(p->end_ns), last);
+        const double bytes = (double)n * E->bkt_rows * ((double)E->bkt_n + 1) * sizeof(hs_bucket) + (double)n * E->bkt_rows * 8.0;
+        size_t free_b = 0, total_b = 0;
+        CUDA_TRY(cudaMemGetInfo(&free_b, &total_b));
+        if (bytes > (double)(free_b + E->d_buckets.n + E->d_bkt_past.n))
+            return fail(HS_ERR_INVALID, "time buckets need %.3f GB (%u replicas x %u rows x %u buckets x 32 B), the device has %.3f GB free",
+                        bytes / 1e9, n, E->bkt_rows, E->bkt_n + 1, (double)(free_b + E->d_buckets.n + E->d_bkt_past.n) / 1e9);
+    }
     int rc;
+    if (bkt_records) {
+        if ((rc = E->d_buckets.ensure(bkt_records * sizeof(hs_bucket)))) return rc;
+        if ((rc = E->d_bkt_past.ensure((size_t)n * E->bkt_rows * 8))) return rc;
+        if (!p->resume) {
+            CUDA_TRY(cudaMemsetAsync(E->d_buckets.p, 0, bkt_records * sizeof(hs_bucket), E->stream));
+            CUDA_TRY(cudaMemsetAsync(E->d_bkt_past.p, 0, (size_t)n * E->bkt_rows * 8, E->stream));
+        }
+    }
     if ((rc = E->d_summ.ensure((size_t)n * sizeof(hs_replica_summary)))) return rc;
     if ((rc = E->d_stats.ensure((size_t)n * ne * sizeof(hs_entity_stats)))) return rc;
     if ((rc = E->d_rec.ensure((size_t)n * p->record_cap * sizeof(hs_event_record)))) return rc;
@@ -755,13 +837,18 @@ int hs_run(hs_engine *E, const hs_run_params *p)
     O.sketch = (uint8_t *)E->d_sketch.p;
     O.outbox = (hs_xevent *)E->d_outbox.p; O.outbox_n = (uint32_t *)E->d_outbox_n.p;
     O.inbox = (hs_xevent *)E->d_inbox.p; O.inbox_n = (uint32_t *)E->d_inbox_n.p;
+    hs_bucket_args BK;
+    BK.w = E->bkt_w; BK.n = E->bkt_n; BK.rows = E->bkt_rows; BK.acc_off = 0; BK.pad = 0;
+    BK.rec = bkt_records ? (hs_bucket *)E->d_buckets.p : nullptr;
+    BK.past_end = bkt_records ? (int64_t *)E->d_bkt_past.p : nullptr;
     const bool want_hash = (p->flags & HS_RUN_ORDER_HASH) != 0;
     const bool want_rec = (p->record_cap | p->sample_cap | p->service_cap) != 0;
-    rc = engine == 2 ? launch_lane(E, R, O, want_hash, want_rec)
-       : engine == 3 ? launch_thread(E, R, O, want_hash, want_rec, linked)
-       : launch_warp(E, R, O, want_hash, want_rec);
+    rc = engine == 2 ? launch_lane(E, R, O, want_hash, want_rec, BK)
+       : engine == 3 ? launch_thread(E, R, O, want_hash, want_rec, linked, BK)
+       : launch_warp(E, R, O, want_hash, want_rec, BK);
     if (rc) return rc;
     E->last = *p;
+    E->last_bkt_w = E->bkt_w; E->last_bkt_n = E->bkt_n;
     E->last_engine = engine;
     E->last_ring = ring;
     E->have_run = true;
@@ -788,6 +875,97 @@ int hs_set_trace(hs_engine *E, const double *arr, uint64_t n_arr, const double *
         E->n_trace_svc = n_svc;
     }
     E->trace_replicas = n_replicas;
+    return HS_OK;
+}
+
+int hs_set_buckets(hs_engine *E, double width_s, uint32_t n)
+{
+    if (!E) return fail(HS_ERR_INVALID, "engine is NULL");
+    if (n && !(width_s > 0.0 && width_s < 1e300)) return fail(HS_ERR_INVALID, "bucket width must be a finite number of seconds > 0, got %g", width_s);
+    if (n > (1u << 24)) return fail(HS_ERR_INVALID, "at most 2^24 buckets per row, got %u", n);
+    E->bkt_w = n ? width_s : 0.0;
+    E->bkt_n = n;
+    return HS_OK;
+}
+
+int hs_read_buckets(hs_engine *E, hs_bucket *out, int64_t *past_end, uint32_t *rows)
+{
+    if (!E) return fail(HS_ERR_INVALID, "engine is NULL");
+    if (!E->have_run) return fail(HS_ERR_STATE, "no run yet");
+    if (rows) *rows = E->bkt_rows;
+    if (!E->last_bkt_n) return fail(HS_ERR_STATE, "the last run had no time buckets (hs_set_buckets)");
+    CUDA_TRY(cudaSetDevice(E->device));
+    const size_t nr = (size_t)E->last.n_replicas * E->bkt_rows;
+    if (out && nr) CUDA_TRY(cudaMemcpyAsync(out, E->d_buckets.p, nr * (E->last_bkt_n + 1u) * sizeof(hs_bucket), cudaMemcpyDeviceToHost, E->stream));
+    if (past_end && nr) CUDA_TRY(cudaMemcpyAsync(past_end, E->d_bkt_past.p, nr * 8, cudaMemcpyDeviceToHost, E->stream));
+    CUDA_TRY(cudaStreamSynchronize(E->stream));
+    return HS_OK;
+}
+
+int hs_read_bucket_totals(hs_engine *E, hs_bucket_total *out, uint32_t n_cells)
+{
+    if (!E || !out || n_cells == 0) return fail(HS_ERR_INVALID, "bad argument");
+    if (!E->have_run) return fail(HS_ERR_STATE, "no run yet");
+    if (!E->last_bkt_n) return fail(HS_ERR_STATE, "the last run had no time buckets (hs_set_buckets)");
+    const hs_run_params &p = E->last;
+    const uint32_t per = E->bkt_rows * (E->last_bkt_n + 1u);
+    if (per == 0) return HS_OK;
+    CUDA_TRY(cudaSetDevice(E->device));
+    /* slices: at most HS_BUCKET_SLICE consecutive replicas of one cell (cell = (global index / replicas_per_cell) % n_cells:
+     * a plain ensemble is one cell, so its slices are 256 replicas each); per cell its slices in index order */
+    std::vector<hs_bucket_slice> slices;
+    std::vector<uint32_t> slice_cell;
+    const auto cell_of = [&](uint64_t r) { return (uint32_t)((((uint64_t)p.replica_index_base + r) / p.replicas_per_cell) % n_cells); };
+    for (uint32_t r = 0; r < p.n_replicas;) {
+        const uint32_t c = cell_of(r);
+        const uint64_t lim = std::min<uint64_t>((uint64_t)r + HS_BUCKET_SLICE, p.n_replicas);
+        uint64_t end = r;
+        while (end < lim && cell_of(end) == c) {     /* whole runs of replicas_per_cell replicas at a time */
+            const uint64_t run = ((uint64_t)p.replica_index_base + end) / p.replicas_per_cell;
+            end = std::min<uint64_t>((run + 1) * p.replicas_per_cell - p.replica_index_base, lim);
+        }
+        slices.push_back({r, (uint32_t)end});
+        slice_cell.push_back(c);
+        r = (uint32_t)end;
+    }
+    std::vector<uint32_t> first(n_cells + 1, 0), order(slices.size());
+    for (uint32_t c : slice_cell) first[c + 1]++;
+    for (uint32_t c = 0; c < n_cells; ++c) first[c + 1] += first[c];
+    {
+        std::vector<uint32_t> at(first.begin(), first.end() - 1);
+        for (uint32_t s = 0; s < (uint32_t)slices.size(); ++s) order[at[slice_cell[s]]++] = s;
+    }
+    const uint32_t ns = (uint32_t)slices.size();
+    const size_t idx_bytes = (size_t)ns * sizeof(hs_bucket_slice) + (first.size() + order.size()) * 4;
+    {
+        const double bytes = ((double)ns + n_cells) * per * sizeof(hs_bucket_total) + (double)idx_bytes;
+        size_t free_b = 0, total_b = 0;
+        CUDA_TRY(cudaMemGetInfo(&free_b, &total_b));
+        const double have = (double)free_b + E->d_bkt_partial.n + E->d_bkt_out.n + E->d_bkt_index.n;
+        if (bytes > have)
+            return fail(HS_ERR_INVALID, "the bucket cell reduction needs %.3f GB (%u slices + %u cells x %u records x 48 B), the device has %.3f GB free",
+                        bytes / 1e9, ns, n_cells, per, have / 1e9);
+    }
+    int rc;
+    if ((rc = E->d_bkt_index.ensure(idx_bytes))) return rc;
+    if ((rc = E->d_bkt_partial.ensure((size_t)ns * per * sizeof(hs_bucket_total)))) return rc;
+    if ((rc = E->d_bkt_out.ensure((size_t)n_cells * per * sizeof(hs_bucket_total)))) return rc;
+    unsigned char *ix = (unsigned char *)E->d_bkt_index.p;
+    const hs_bucket_slice *d_slices = (const hs_bucket_slice *)ix;
+    const uint32_t *d_first = (const uint32_t *)(ix + (size_t)ns * sizeof(hs_bucket_slice));
+    const uint32_t *d_order = d_first + first.size();
+    CUDA_TRY(cudaMemcpyAsync(ix, slices.data(), (size_t)ns * sizeof(hs_bucket_slice), cudaMemcpyHostToDevice, E->stream));
+    CUDA_TRY(cudaMemcpyAsync((void *)d_first, first.data(), first.size() * 4, cudaMemcpyHostToDevice, E->stream));
+    CUDA_TRY(cudaMemcpyAsync((void *)d_order, order.data(), order.size() * 4, cudaMemcpyHostToDevice, E->stream));
+    const dim3 g1((per + 127) / 128, std::min<uint32_t>(ns, 65535u)), g2((per + 127) / 128, std::min<uint32_t>(n_cells, 65535u));
+    hs_bucket_partial_kernel<<<g1, 128, 0, E->stream>>>((const hs_bucket *)E->d_buckets.p, per, d_slices, ns, (hs_bucket_total *)E->d_bkt_partial.p);
+    CUDA_TRY(cudaGetLastError());
+    hs_bucket_final_kernel<<<g2, 128, 0, E->stream>>>((const hs_bucket_total *)E->d_bkt_partial.p, per, d_first, d_order, n_cells,
+                                                      (hs_bucket_total *)E->d_bkt_out.p);
+    CUDA_TRY(cudaGetLastError());
+    E->launches += 2;
+    CUDA_TRY(cudaMemcpyAsync(out, E->d_bkt_out.p, (size_t)n_cells * per * sizeof(hs_bucket_total), cudaMemcpyDeviceToHost, E->stream));
+    CUDA_TRY(cudaStreamSynchronize(E->stream));   /* the host vectors above are the copies' sources */
     return HS_OK;
 }
 

@@ -65,6 +65,7 @@
 #include "hs_sampler.h"
 #include "hs_profile.h"
 #include "hs_kernel_params.cuh"
+#include "hs_buckets.cuh"
 
 #define HS_NOW_CAP 8
 #define HS_LANE_THREADS 64
@@ -77,6 +78,8 @@
 #define HS_LF_PROFILE 4   /* non-constant rate profile (Simpson + Brent path) */
 #define HS_LF_SIMPLE 8    /* compile-time model: Poisson source without stop_after, exponential FIFO server with an
                              unbounded queue, Sink downstream, Philox draws -- the BASELINE configs[0]/[1] shape */
+#define HS_LF_BUCKETS 16  /* time buckets of the Sink samples (hs_set_buckets; the Sink is bucketed row 0); compiled
+                             without HS_LF_REC only */
 
 struct hs_now_ev {        /* an event created at the current timestamp       */
     uint64_t idx;         /* Event._sort_index                               */
@@ -150,7 +153,8 @@ __device__ __forceinline__ int64_t hs_lane_next_arrival(int64_t t, double target
 template <int FLAGS>
 __global__ void __launch_bounds__(HS_LANE_THREADS, 7)
 hs_lane_kernel(hs_lane_model M, hs_kernel_run P, hs_lane_state *__restrict__ states,
-               hs_ring_entry *__restrict__ rings, hs_cont *__restrict__ conts, hs_kernel_out O)
+               hs_ring_entry *__restrict__ rings, hs_cont *__restrict__ conts, hs_kernel_out O,
+               typename hs_bucket_args_of<(FLAGS & HS_LF_BUCKETS) != 0>::type BK)
 {
     constexpr uint32_t HS_DRAW_BUF = (FLAGS & HS_LF_REC) ? HS_DRAW_BUF_RECORD : HS_DRAW_BUF_SUMMARY;
     constexpr uint32_t STAGE_ROWS = (FLAGS & HS_LF_REC) ? HS_STAGE : 1;
@@ -233,6 +237,9 @@ hs_lane_kernel(hs_lane_model M, hs_kernel_run P, hs_lane_state *__restrict__ sta
     const bool svc_quads = (FLAGS & HS_LF_REC) && (P.service_cap % 4u) == 0;
     bool smp_sync = false, svc_sync = false;
     hs_now_ev nowq[HS_NOW_CAP];
+    /* the Sink's current time bucket (HS_LF_BUCKETS; an empty type otherwise): stored when it moves on and at the end */
+    typename hs_bucket_acc_of<(FLAGS & HS_LF_BUCKETS) != 0>::type bacc;
+    if (FLAGS & HS_LF_BUCKETS) hs_bucket_reset(bacc);
 
     hs_lane_state *S = states + r;
     bool finished = !valid;
@@ -384,6 +391,7 @@ hs_lane_kernel(hs_lane_model M, hs_kernel_run P, hs_lane_state *__restrict__ sta
             hs_neumaier_add(&sum, &comp, lat_); sumsq = HS_ADD(sumsq, HS_MUL(lat_, lat_));   \
             if (lat_ < mn) mn = lat_;                                                        \
             if (lat_ > mx) mx = lat_;                                                        \
+            if (FLAGS & HS_LF_BUCKETS) hs_bucket_add(BK, r, 0u, bacc, now, lat_);          \
             if ((FLAGS & HS_LF_REC) && smp) {                                                \
                 uint4 w_; const uint64_t lb_ = (uint64_t)__double_as_longlong(lat_);         \
                 w_.x = (uint32_t)(uint64_t)now; w_.y = (uint32_t)((uint64_t)now >> 32);      \
@@ -616,6 +624,7 @@ hs_lane_kernel(hs_lane_model M, hs_kernel_run P, hs_lane_state *__restrict__ sta
                     sumsq = isC ? q2_ : sumsq;
                     mn = (isC && lat_ < mn) ? lat_ : mn;
                     mx = (isC && lat_ > mx) ? lat_ : mx;
+                    if (isC && (FLAGS & HS_LF_BUCKETS)) hs_bucket_add(BK, r, 0u, bacc, now, lat_);
                     if (isC && (FLAGS & HS_LF_REC) && smp) {
                         uint4 w_; const uint64_t lb_ = (uint64_t)__double_as_longlong(lat_);
                         w_.x = (uint32_t)(uint64_t)now; w_.y = (uint32_t)((uint64_t)now >> 32);
@@ -841,6 +850,7 @@ hs_lane_kernel(hs_lane_model M, hs_kernel_run P, hs_lane_state *__restrict__ sta
 
     if (!valid) return;
     if (P.resume && S->done) return;        /* finished in an earlier window: outputs already final */
+    if (FLAGS & HS_LF_BUCKETS) hs_bucket_flush(BK, r, 0u, bacc);   /* the current time bucket, at the run's end or a pause */
     if ((FLAGS & HS_LF_REC) && staged) {    /* drain what is still staged, record by record */
         while (st_fl != st_wr) {
             __stcs((uint4 *)(rec + rec_pos), sh_rec[st_fl % HS_STAGE][tid]);

@@ -81,7 +81,8 @@ __device__ __forceinline__ void hs_prefetch(const void *p) { asm volatile("prefe
 template <int FLAGS>
 __device__ __forceinline__ void
 hs_thread_body(const hs_warp_model &M, const hs_kernel_run &P, unsigned char *__restrict__ blocks,
-               hs_wring_entry *__restrict__ rings, const hs_kernel_out &O)
+               hs_wring_entry *__restrict__ rings, const hs_kernel_out &O,
+               const typename hs_bucket_args_of<(FLAGS & HS_WF_BUCKETS) != 0>::type BK)
 {
     /* dynamic shared memory of a block: [ now tier: HS_T_KS x 3 chunks x rpb columns | heap top: P.heap_top keys x rpb columns ],
      * rpb = replicas (columns) of the block.  The now tier is sized by the columns in use (it was 64 wide whatever the
@@ -110,6 +111,7 @@ hs_thread_body(const hs_warp_model &M, const hs_kernel_run &P, unsigned char *__
     auto pay_at = [&](const uint32_t slot) -> hs_tpay * { return M.fixed_slots ? &E[slot].pay : &PAY[slot]; };
     uint16_t *FREE = (uint16_t *)(blk + L.free_);
     hs_wnow *Ng = (hs_wnow *)(blk + L.spill);
+    auto *const bacc = hs_bucket_accs(BK, blk);          /* HS_WF_BUCKETS: the rows' current time buckets, after the block's own layout */
 
     /* Heap keys: the first P.heap_top (whole top levels) live in shared memory for the duration of the launch -- a pop's
      * sift-down walks the top of the heap every time, and in global memory every level is a dependent L2/DRAM round
@@ -239,6 +241,7 @@ hs_thread_body(const hs_warp_model &M, const hs_kernel_run &P, unsigned char *__
     hs_event_record *rec = (FLAGS & HS_WF_REC) && O.records ? O.records + (size_t)r * P.record_cap : nullptr;
     hs_sink_sample *smp = (FLAGS & HS_WF_REC) && O.samples ? O.samples + (size_t)r * P.sample_cap : nullptr;
     double *svc_out = (FLAGS & HS_WF_REC) && O.service ? O.service + (size_t)r * P.service_cap : nullptr;
+    hs_bucket_begin(BK, bacc);
 
     /* the header's hot fields live in registers for the duration of the launch (the struct itself is addressed through
      * H by the handlers, i.e. it sits in local memory) and are written back with it at the end */
@@ -562,6 +565,7 @@ hs_thread_body(const hs_warp_model &M, const hs_kernel_run &P, unsigned char *__
                     Xk->u.snk.sumsq = HS_ADD(Xk->u.snk.sumsq, HS_MUL(lat, lat));
                     if (lat < Xk->u.snk.mn) Xk->u.snk.mn = lat;
                     if (lat > Xk->u.snk.mx) Xk->u.snk.mx = lat;
+                    if (FLAGS & HS_WF_BUCKETS) hs_bucket_add(BK, r, (uint32_t)__double_as_longlong(ENTS[tgt].d1), bacc, now, lat);
                     if ((FLAGS & HS_WF_REC) && smp) { hs_sink_sample qs; qs.completion_ns = now; qs.latency_s = lat; smp[hdr.smp_pos] = qs;
                         hdr.smp_pos = (hdr.smp_pos + 1 == P.sample_cap) ? 0u : hdr.smp_pos + 1; }
                     hdr.n_smp++;
@@ -797,6 +801,7 @@ hs_thread_body(const hs_warp_model &M, const hs_kernel_run &P, unsigned char *__
     H->now = h_now; H->processed = h_processed; H->hash = h_hash; H->fel_n = h_fel;
     hdr.done = paused ? 0 : 1;
     *Hg = hdr;
+    hs_bucket_end(BK, r, bacc);                          /* every row's current time bucket, at the run's end or a pause */
     if (O.summaries) {
         hs_replica_summary s;
         s.events_processed = h_processed; s.final_time_ns = h_now;
@@ -820,7 +825,7 @@ __global__ void __launch_bounds__(HS_THREAD_BLOCK, HS_T_MINBLOCKS)
 hs_thread_kernel(hs_warp_model M, hs_kernel_run P, unsigned char *__restrict__ blocks,
                  hs_wring_entry *__restrict__ rings, hs_kernel_out O)
 {
-    hs_thread_body<FLAGS>(M, P, blocks, rings, O);
+    hs_thread_body<FLAGS>(M, P, blocks, rings, O, hs_no_bucket_args());
 }
 
 #define HS_T_WIDE_BLOCKS 4
@@ -829,7 +834,25 @@ __global__ void __launch_bounds__(HS_THREAD_BLOCK, HS_T_WIDE_BLOCKS)
 hs_thread_kernel_wide(hs_warp_model M, hs_kernel_run P, unsigned char *__restrict__ blocks,
                       hs_wring_entry *__restrict__ rings, hs_kernel_out O)
 {
-    hs_thread_body<FLAGS>(M, P, blocks, rings, O);
+    hs_thread_body<FLAGS>(M, P, blocks, rings, O, hs_no_bucket_args());
+}
+
+/* the same two entry points for the time-bucket instantiations (FLAGS with HS_WF_BUCKETS): the bucket arguments come
+ * as one more parameter, which the kernels above do not have */
+template <int FLAGS>
+__global__ void __launch_bounds__(HS_THREAD_BLOCK, HS_T_MINBLOCKS)
+hs_thread_bucket_kernel(hs_warp_model M, hs_kernel_run P, unsigned char *__restrict__ blocks,
+                        hs_wring_entry *__restrict__ rings, hs_kernel_out O, hs_bucket_args BK)
+{
+    hs_thread_body<FLAGS>(M, P, blocks, rings, O, BK);
+}
+
+template <int FLAGS>
+__global__ void __launch_bounds__(HS_THREAD_BLOCK, HS_T_WIDE_BLOCKS)
+hs_thread_bucket_kernel_wide(hs_warp_model M, hs_kernel_run P, unsigned char *__restrict__ blocks,
+                             hs_wring_entry *__restrict__ rings, hs_kernel_out O, hs_bucket_args BK)
+{
+    hs_thread_body<FLAGS>(M, P, blocks, rings, O, BK);
 }
 
 #endif /* HS_THREAD_ENGINE_CUH */

@@ -32,6 +32,7 @@
 #include "hs_profile.h"
 #include "hs_sketch.h"
 #include "hs_kernel_params.cuh"
+#include "hs_buckets.cuh"
 
 #define HS_WF_HASH 1
 #define HS_WF_REC 2
@@ -41,6 +42,8 @@
                               launch, finished replicas run on, tie detection); compiled out of every other launch */
 #define HS_WF_FAULTS 32    /* the model has FAULT rows (node faults): their bootstrap, the crashed-entity drop, cancelled pops and
                               the tie test; compiled out of every other launch */
+#define HS_WF_BUCKETS 64   /* time buckets of the Sink / Probe samples (hs_set_buckets, hs_buckets.cuh); compiled out of every
+                              other launch.  The row of a SINK / PROBE entity is the low word of its device row's d1 */
 
 struct __align__(16) hs_warp_hdr {      /* 128 B */
     int64_t now; uint64_t ctr; int64_t processed; uint64_t hash;
@@ -208,7 +211,8 @@ __device__ __forceinline__ void hs_tma_store_1d(void *gmem_dst, const void *smem
 template <int FLAGS>
 __global__ void __launch_bounds__(256)
 hs_warp_kernel(hs_warp_model M, hs_kernel_run P, unsigned char *__restrict__ blocks,
-               hs_wring_entry *__restrict__ rings, hs_kernel_out O, unsigned int *__restrict__ next_replica)
+               hs_wring_entry *__restrict__ rings, hs_kernel_out O, unsigned int *__restrict__ next_replica,
+               typename hs_bucket_args_of<(FLAGS & HS_WF_BUCKETS) != 0>::type BK)
 {
     extern __shared__ __align__(16) unsigned char smem_raw[];
     const int lane = threadIdx.x & 31;
@@ -327,6 +331,8 @@ hs_warp_kernel(hs_warp_model M, hs_kernel_run P, unsigned char *__restrict__ blo
         hs_event_record *rec = (FLAGS & HS_WF_REC) && O.records ? O.records + (size_t)r * P.record_cap : nullptr;
         hs_sink_sample *smp = (FLAGS & HS_WF_REC) && O.samples ? O.samples + (size_t)r * P.sample_cap : nullptr;
         double *svc_out = (FLAGS & HS_WF_REC) && O.service ? O.service + (size_t)r * P.service_cap : nullptr;
+        auto *const bacc = hs_bucket_accs(BK, blk);     /* HS_WF_BUCKETS: the rows' current time buckets, in the staged block */
+        if (lane == 0) hs_bucket_begin(BK, bacc);
 
         /* ---- pop-invoke-push --------------------------------------------------- */
         bool paused = false;
@@ -453,6 +459,7 @@ hs_warp_kernel(hs_warp_model M, hs_kernel_run P, unsigned char *__restrict__ blo
 
         /* ---- publish + write the block back -------------------------------- */
         if (lane == 0) {
+            hs_bucket_end(BK, r, bacc);                 /* every row's current time bucket, at the run's end or a pause */
             H->done = paused ? 0 : 1;
             if (O.summaries) {
                 hs_replica_summary s;

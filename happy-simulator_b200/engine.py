@@ -30,7 +30,8 @@ EXPORTED_SYMBOLS = ["hs_version", "hs_last_error", "hs_engine_create", "hs_engin
                     "hs_last_launch", "hs_read_outputs", "hs_read_totals", "hs_read_cell_totals", "hs_totals_device_ptr",
                     "hs_sketch_layout", "hs_read_sketches", "hs_coordinator_create", "hs_coordinator_destroy",
                     "hs_coordinator_exchange", "hs_coordinator_read", "hs_read_outbox", "hs_read_inbox",
-                    "hs_partition_upload", "hs_partition_validate"]
+                    "hs_partition_upload", "hs_partition_validate", "hs_set_buckets", "hs_read_buckets",
+                    "hs_read_bucket_totals"]
 
 
 def load_library(path: str | None = None):
@@ -77,6 +78,9 @@ def load_library(path: str | None = None):
         "hs_coordinator_read": ([H, C.POINTER(C.c_uint64), C.POINTER(C.c_uint64), C.POINTER(C.c_uint64)], C.c_int),
         "hs_read_outbox": ([H, C.c_void_p, C.POINTER(C.c_uint32)], C.c_int),
         "hs_read_inbox": ([H, C.c_void_p, C.POINTER(C.c_uint32)], C.c_int),
+        "hs_set_buckets": ([H, C.c_double, C.c_uint32], C.c_int),
+        "hs_read_buckets": ([H, C.c_void_p, C.c_void_p, C.POINTER(C.c_uint32)], C.c_int),
+        "hs_read_bucket_totals": ([H, C.c_void_p, C.c_uint32], C.c_int),
     }
     for name, (args, res) in sigs.items():
         fn = getattr(L, name)
@@ -190,6 +194,26 @@ class Engine:
         assert a.ndim == 2 and s.ndim == 2 and a.shape[0] == s.shape[0]
         _check(self._L, self._L.hs_set_trace(self._h, a.ctypes.data_as(C.POINTER(C.c_double)), a.shape[1],
                                              s.ctypes.data_as(C.POINTER(C.c_double)), s.shape[1], a.shape[0]))
+
+    def set_buckets(self, width_s: float = 0.0, n: int = 0) -> None:
+        """hs_set_buckets: time buckets of width_s seconds, n per row, for the following runs (n = 0: off)."""
+        _check(self._L, self._L.hs_set_buckets(self._h, float(width_s), int(n)))
+
+    def read_buckets(self, n: int):
+        """(BUCKET_DTYPE [n_replicas, rows, n + 1], int64 past-end index [n_replicas, rows]) of the last run, which had
+        n buckets per row (hs_read_buckets)."""
+        rows = C.c_uint32()
+        _check(self._L, self._L.hs_read_buckets(self._h, None, None, C.byref(rows)))
+        nr, nb = int(self._params.n_replicas), int(rows.value)
+        buf, past = np.zeros((nr, nb, n + 1), A.BUCKET_DTYPE), np.zeros((nr, nb), np.int64)
+        _check(self._L, self._L.hs_read_buckets(self._h, buf.ctypes.data, past.ctypes.data, None))
+        return buf, past
+
+    def read_bucket_totals(self, n_cells: int, rows: int, n: int):
+        """BUCKET_TOTAL_DTYPE [n_cells, rows, n + 1]: the last run's buckets reduced per sweep cell (hs_read_bucket_totals)."""
+        out = np.zeros((n_cells, rows, n + 1), A.BUCKET_TOTAL_DTYPE)
+        _check(self._L, self._L.hs_read_bucket_totals(self._h, out.ctypes.data, n_cells))
+        return out
 
     def read_box(self, which: str = "outbox"):
         """(entries XEVENT_DTYPE[n_replicas, cap], counts uint32[n_replicas]) of the partition's outbox / inbox."""

@@ -28,7 +28,7 @@
 extern "C" {
 #endif
 
-#define HS_ABI_VERSION 6u
+#define HS_ABI_VERSION 7u
 
 typedef enum hs_status {
     HS_OK = 0,
@@ -338,6 +338,28 @@ typedef struct hs_cell_totals {
     uint64_t histogram[HS_HISTOGRAM_BINS];
 } hs_cell_totals;
 
+/* Time buckets (hs_set_buckets): the reference's Data.bucket(window_s) (instrumentation/data.py:127-158) of every
+ * replica's Sink / LatencyTracker / ThroughputTracker / Probe samples, reduced on the device as the samples arrive.
+ * The bucketed rows are the model's SINK and PROBE rows in entity order (row b = the b-th of them).  A sample at t ns
+ * with value v (a Sink's latency in seconds, a Probe's metric) goes to bucket k = floor((t / 1e9) / width_s), both
+ * divisions correctly rounded, as math.floor(Instant.to_seconds() / window_s) computes it. */
+typedef struct hs_bucket {         /* one bucket of one row of one replica, 32 bytes                        */
+    int64_t count;                 /* samples in the bucket (0: the bucket is empty, Data.bucket omits it)   */
+    double sum, comp;              /* sum(values) as CPython's float sum() computes it: sum + comp (Neumaier) */
+    double max;                    /* max(values); meaningless when count == 0                              */
+} hs_bucket;
+
+/* One bucket of one row over the replicas of one sweep cell, 48 bytes.  Summed in a fixed order (replicas in index
+ * order within slices of at most 256 that do not cross a cell boundary, then the slices in index order), with no
+ * atomics: repeated runs give the same bits whichever engine ran the replicas. */
+typedef struct hs_bucket_total {
+    int64_t replicas;              /* replicas with at least one sample in the bucket                         */
+    int64_t count;                 /* sum of their counts                                                     */
+    double sum;                    /* sum of their bucket sums (sum + comp each)                              */
+    double mean_sum, mean_sq_sum;  /* sum of their bucket means (sum / count) and of the squared means        */
+    double max;                    /* max of their maxes (-inf if replicas == 0)                              */
+} hs_bucket_total;
+
 /* ---- entry points ------------------------------------------------------ */
 
 typedef struct hs_engine hs_engine;
@@ -481,6 +503,26 @@ int hs_coordinator_read(hs_coordinator *c, uint64_t *delivered, uint64_t *lost, 
 /* Copy the current outboxes / inboxes to the host: buf[n_replicas][cap], counts[n_replicas] (tests, debugging). */
 int hs_read_outbox(hs_engine *e, hs_xevent *buf, uint32_t *counts);
 int hs_read_inbox(hs_engine *e, hs_xevent *buf, uint32_t *counts);
+
+/* Time buckets for the following hs_run calls: width_s > 0 seconds, n buckets per row and replica (n = 0: off, the
+ * default).  Per replica the engine keeps [rows][n + 1] hs_bucket records: slot k < n is bucket k, slot n holds the
+ * samples with an index >= n (only the one event a replica processes past end_ns can make one; its index is kept
+ * separately).  hs_run refuses a bucketed run whose end time falls into bucket n or later (n * width_s must exceed
+ * the end time), a run with recorder rings (record_cap, sample_cap or service_cap: buckets are the summary-mode
+ * series; the rings stay the record-mode path), a window of a linked partition (HS_RUN_LINKED or a model with
+ * REMOTE rows), and a resume whose bucket configuration differs from the paused run's.  It checks the size of the
+ * records against the free device memory before it allocates them. */
+int hs_set_buckets(hs_engine *e, double width_s, uint32_t n);
+
+/* Copy the last run's buckets: out[n_replicas][rows][n + 1] (see hs_set_buckets) and past_end[n_replicas][rows], the
+ * index of the samples in slot n (valid where that slot's count > 0).  Either pointer may be NULL.  *rows (if not
+ * NULL) receives the number of bucketed rows. */
+int hs_read_buckets(hs_engine *e, hs_bucket *out, int64_t *past_end, uint32_t *rows);
+
+/* Reduce the last run's buckets per sweep cell (cell = global replica index / replicas_per_cell, modulo n_cells, as
+ * hs_read_cell_totals) on the device and copy out[n_cells][rows][n + 1] to the host.  Slot n aggregates the
+ * past-end samples whatever their index. */
+int hs_read_bucket_totals(hs_engine *e, hs_bucket_total *out, uint32_t n_cells);
 
 /* Device pointer/size of the last run's totals (for the NCCL allreduce done by
  * the host layer on torch.distributed; layout = hs_totals). */
