@@ -33,6 +33,7 @@ HS_RUN_LINKED = 4
 HS_ST_LINK_OVERFLOW = 64
 HS_ST_LINK_TIE = 128
 HS_ST_FAULT_TIE = 256
+HS_ST_BUCKET_OVERFLOW = 512
 
 HS_STREAM_ARRIVAL, HS_STREAM_SERVICE, HS_STREAM_ROUTING, HS_STREAM_LINK_LOSS, HS_STREAM_LINK_LATENCY = 0, 1, 2, 3, 4
 
@@ -155,6 +156,9 @@ BUCKET_DTYPE = _np.dtype([("count", "<i8"), ("sum", "<f8"), ("comp", "<f8"), ("m
 BUCKET_TOTAL_DTYPE = _np.dtype([("replicas", "<i8"), ("count", "<i8"), ("sum", "<f8"), ("mean_sum", "<f8"),
                                 ("mean_sq_sum", "<f8"), ("max", "<f8")])
 assert BUCKET_DTYPE.itemsize == 32 and BUCKET_TOTAL_DTYPE.itemsize == 48
+# bucket percentiles (hs_set_bucket_percentiles): hs_bucket_pct_total, 32 bytes
+BUCKET_PCT_TOTAL_DTYPE = _np.dtype([("p50_sum", "<f8"), ("p50_sq_sum", "<f8"), ("p99_sum", "<f8"), ("p99_sq_sum", "<f8")])
+assert BUCKET_PCT_TOTAL_DTYPE.itemsize == 32
 PROFILE_DTYPE = _np.dtype([("kind", "<i4"), ("pad", "<i4"), ("p", "<f8", (4,))])
 assert PROFILE_DTYPE.itemsize == 40
 

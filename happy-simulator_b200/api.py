@@ -799,7 +799,8 @@ class Simulation:
     def run_ensemble(self, n_replicas: int, *, seed: int | None = None, seed_stride: int = 0, rid_base: int = 0,
                      rid_stride: int = 1, replica_index_base: int = 0, replicas_per_cell: int = 1,
                      window_end_s: float | None = None, resume: bool = False, host: dict | None = None,
-                     upload: bool = True, totals: bool = True, on_overflow: str = "grow", buckets=None, **caps):
+                     upload: bool = True, totals: bool = True, on_overflow: str = "grow", buckets=None,
+                     bucket_percentiles: bool = False, bucket_sample_cap: int = 64, **caps):
         """N independent replicas of this model on the device; returns the raw per-replica arrays
         (summaries, entity_stats, optional recorder rings) and the engine's totals.
 
@@ -820,8 +821,17 @@ class Simulation:
         ``buckets.bucketed_data(out, obj, replica)`` gives one replica's ``BucketedData``.  A bucketed run has no
         recorder rings; every window of a windowed run passes the same ``buckets``, and only the window that reaches the
         end time reads them back (the records are gigabytes at full size; ``Engine.read_buckets`` reads them after any
-        window)."""
+        window).
+
+        ``bucket_percentiles=True`` (with ``buckets``) adds every bucket's p50 and p99, bit for bit those of
+        ``Data.bucket(width_s)``: ``out["bucket_percentiles"]`` (float64 [replica, row, n + 1, 2]) and
+        ``out["bucket_percentile_totals"]`` (BUCKET_PCT_TOTAL_DTYPE [cell, row, n + 1]).  The device holds the values of
+        each row's current bucket, at most ``bucket_sample_cap`` of them; a bucket with more samples is handled per
+        ``on_overflow``: "grow" re-runs the ensemble once with the next power of two at or above the largest bucket
+        count (fresh, unwindowed runs only), "raise" and a windowed or resumed run raise ``EnsembleStatusError`` naming
+        the capacity to pass, "ignore" returns NaN for those buckets and the HS_ST_BUCKET_OVERFLOW status bit."""
         spec = _buckets.check_spec(buckets, self._end_time.nanoseconds) if buckets is not None else None
+        cap = _buckets.check_sample_cap(bucket_sample_cap, spec) if bucket_percentiles else 0
         eng = _engine(self._device)
         if lowering.refresh_fault_cancellation(self.model) and not upload and not resume:
             upload = True                   # a FaultHandle was cancelled since the last upload
@@ -836,9 +846,22 @@ class Simulation:
             we = w if w < end_ns else -1
         ring = int(caps.pop("queue_ring", 0) or 0)
         eng.set_buckets(*(spec or (0.0, 0)))
+        eng.set_bucket_percentiles(cap)
         try:
-            out, st, ring = self._run_windows(eng, n_replicas, seed, seed_stride, rid_base, rid_stride, replica_index_base,
-                                              replicas_per_cell, end_ns, we, resume, ring, host, on_overflow, caps)
+            run = (eng, n_replicas, seed, seed_stride, rid_base, rid_stride, replica_index_base, replicas_per_cell, end_ns,
+                   we, resume)
+            out, st, ring = self._run_windows(*run, ring, host, on_overflow, caps)
+            if cap and on_overflow != "ignore" and int(np.bitwise_or.reduce(st)) & A.HS_ST_BUCKET_OVERFLOW:
+                need = _buckets.sample_cap_needed(eng.read_buckets(spec[1])[0])
+                if on_overflow == "grow" and not resume and we < 0:
+                    cap = need
+                    eng.set_bucket_percentiles(cap)
+                    out, st, ring = self._run_windows(*run, ring, host, on_overflow, caps)
+                if int(np.bitwise_or.reduce(st)) & A.HS_ST_BUCKET_OVERFLOW:
+                    n_over = int((st & A.HS_ST_BUCKET_OVERFLOW != 0).sum())
+                    raise EnsembleStatusError(f"{n_over} of {n_replicas} replicas had a time bucket with more samples than "
+                                              f"bucket_sample_cap={cap}; pass bucket_sample_cap={need}"
+                                              + (" (or more: later windows may need it)" if we >= 0 else ""), st.copy())
             if spec and we < 0:
                 w, nb = spec
                 out["buckets"], out["bucket_past_end"] = eng.read_buckets(nb)
@@ -847,8 +870,13 @@ class Simulation:
                 out["bucket_width_s"], out["bucket_count"] = w, nb
                 out["bucket_rows"] = _buckets.rows(self.model)
                 out["bucket_objects"] = _buckets.row_objects(self.model, self.objects)
+                if cap:
+                    out["bucket_percentiles"] = eng.read_bucket_percentiles(nb)
+                    out["bucket_percentile_totals"] = eng.read_bucket_percentile_totals(n_cells, out["buckets"].shape[1], nb)
+                    out["bucket_sample_cap"] = cap
         finally:
-            eng.set_buckets(0.0, 0)             # the engine is shared: other runs get no buckets unless they ask
+            eng.set_bucket_percentiles(0)       # the engine is shared: other runs get no buckets unless they ask
+            eng.set_buckets(0.0, 0)
         out["status"] = st
         out["queue_ring"] = ring
         if totals:
@@ -1105,7 +1133,8 @@ class ParallelRunner:
     def run_replicas(self, build_fn: Callable, n_replicas: int, base_seed: int = 42, **caps):
         """Returns a list-like of ParallelResult (materialised on access).  Device queue rings that overflow
         are grown and the ensemble re-run (``Simulation.run_ensemble``); every result carries ``status``.
-        ``buckets=(width_s, n)`` goes to ``run_ensemble``: the time buckets are in the returned list's ``.raw``."""
+        ``buckets=(width_s, n)``, ``bucket_percentiles`` and ``bucket_sample_cap`` go to ``run_ensemble``: the time
+        buckets are in the returned list's ``.raw``."""
         sim = build_fn()
         t0 = _time.monotonic()
         out = sim.run_ensemble(n_replicas, seed=base_seed, seed_stride=1, rid_base=sim._replica, rid_stride=0,

@@ -2,9 +2,10 @@
 
 ``Simulation.run_ensemble(..., buckets=(width_s, n))`` has the device reduce every replica's samples into the
 reference's ``Data.bucket(width_s)`` (instrumentation/data.py:127-158) as they arrive -- count, ``sum()``, ``max()``
-per bucket -- instead of recording the samples, and reduces those per sweep cell.  This module holds the host side:
-the argument check, the bucket index restated on the host, the row -> object mapping, the reference's
-``BucketedData`` of one object of one replica, and a numpy restatement of the device's cell reduction."""
+per bucket -- instead of recording the samples, and reduces those per sweep cell.  With ``bucket_percentiles=True`` it
+also selects every bucket's p50 and p99 from the current bucket's values.  This module holds the host side: the
+argument checks, the bucket index restated on the host, the row -> object mapping, the reference's ``BucketedData`` of
+one object of one replica, and numpy restatements of the device's cell reductions."""
 from __future__ import annotations
 
 import math
@@ -15,6 +16,7 @@ from . import _abi as A
 from .instrumentation import BucketedData
 
 MAX_BUCKETS = 1 << 24
+MAX_SAMPLE_CAP = 1 << 24
 SLICE = 256                 # replicas per first-stage slice of the cell reduction (HS_BUCKET_SLICE)
 
 
@@ -38,6 +40,22 @@ def check_spec(buckets, end_ns: int) -> tuple[float, int]:
         raise ValueError(f"{n} buckets of {w} s end before the end time {int(end_ns) / 1e9} s (it falls in bucket {last}): "
                          "n * width must exceed the end time")
     return w, n
+
+
+def check_sample_cap(cap, spec) -> int:
+    """``bucket_sample_cap`` of a ``bucket_percentiles=True`` run: an int in [1, 2^24], and buckets to go with it."""
+    if spec is None:
+        raise ValueError("bucket_percentiles=True needs buckets=(width_s, n)")
+    if isinstance(cap, bool) or not isinstance(cap, (int, np.integer)) or not 1 <= int(cap) <= MAX_SAMPLE_CAP:
+        raise ValueError(f"bucket_sample_cap must be an int in [1, 2^24], got {cap!r}")
+    return int(cap)
+
+
+def sample_cap_needed(rec) -> int:
+    """The sample capacity that holds every bucket of the records ``rec`` (BUCKET_DTYPE): the next power of two at or
+    above the largest count."""
+    top = max(1, int(rec["count"].max(initial=1)))
+    return min(MAX_SAMPLE_CAP, 1 << (top - 1).bit_length())
 
 
 def bucket_index(ns, w: float):
@@ -84,8 +102,14 @@ def replica_sums(rec):
 def bucketed_data(out, obj, replica: int) -> BucketedData:
     """The reference's ``Data.bucket(width_s)`` of ``obj`` (a Sink, LatencyTracker, ThroughputTracker, Probe or a
     Probe's Data) in replica ``replica`` of a bucketed ``run_ensemble`` result ``out``.  Times, means, counts, maxes
-    and sums are those of the replica's complete sample list; p50 and p99 need the samples and are NaN (record mode,
-    ``sample_cap``, keeps them for small runs).  Empty buckets are omitted, as Data.bucket omits them."""
+    and sums are those of the replica's complete sample list.  p50 and p99 are those of ``bucket_percentiles=True``
+    (NaN for a bucket that overflowed its sample capacity); without it they are NaN (record mode, ``sample_cap``, keeps
+    the samples for small runs).  Empty buckets are omitted, as Data.bucket omits them.
+
+    A ThroughputTracker's samples are all 1.0, so its sums, maxes and percentiles are derived here from the counts.
+    The device does not know which rows are ThroughputTracker rows: its records, ``out["bucket_percentiles"]``, and
+    the per-cell ``out["bucket_totals"]`` / ``out["bucket_percentile_totals"]`` of such a row are over the latencies
+    the tracker received, raw device values."""
     b = _row_of(out, obj)
     w, n = out["bucket_width_s"], out["bucket_count"]
     rec = out["buckets"][replica, b]
@@ -94,6 +118,7 @@ def bucketed_data(out, obj, replica: int) -> BucketedData:
     slots = keys + ([n] if rec["count"][n] > 0 else [])
     one = _is_throughput(out["bucket_objects"][b])
     sums = replica_sums(rec)
+    pct = out["bucket_percentiles"][replica, b] if "bucket_percentiles" in out else None
     res = BucketedData()
     for k, s in zip(idx, slots):
         c = int(rec["count"][s])
@@ -103,9 +128,27 @@ def bucketed_data(out, obj, replica: int) -> BucketedData:
         res._counts.append(c)
         res._maxes.append(1.0 if one else float(rec["max"][s]))
         res._sums.append(total)
-        res._p50s.append(math.nan)
-        res._p99s.append(math.nan)
+        if pct is None:
+            res._p50s.append(math.nan)
+            res._p99s.append(math.nan)
+        else:                                               # 1.0 * (1 - f) + 1.0 * f rounds to 1.0 for every f
+            res._p50s.append(1.0 if one and not math.isnan(pct[s, 0]) else float(pct[s, 0]))
+            res._p99s.append(1.0 if one and not math.isnan(pct[s, 1]) else float(pct[s, 1]))
     return res
+
+
+def _cell_slices(nr: int, n_cells: int, replica_index_base: int, replicas_per_cell: int):
+    """The device's slices (hs_read_bucket_totals): (cell, begin, end) for runs of at most 256 consecutive replicas of
+    one cell, in index order."""
+    cell_of = ((replica_index_base + np.arange(nr)) // replicas_per_cell) % n_cells
+    r = 0
+    while r < nr:
+        c0 = int(cell_of[r])
+        end = r + 1
+        while end < min(r + SLICE, nr) and cell_of[end] == c0:
+            end += 1
+        yield c0, r, end
+        r = end
 
 
 def cell_totals_reference(buckets, n_cells: int, *, replica_index_base: int = 0, replicas_per_cell: int = 1):
@@ -117,13 +160,7 @@ def cell_totals_reference(buckets, n_cells: int, *, replica_index_base: int = 0,
     out = np.zeros((n_cells,) + shape, A.BUCKET_TOTAL_DTYPE)
     out["max"] = -np.inf
     fields = ("sum", "mean_sum", "mean_sq_sum")
-    cell_of = ((replica_index_base + np.arange(nr)) // replicas_per_cell) % n_cells
-    r = 0
-    while r < nr:
-        c0 = int(cell_of[r])
-        end = r + 1
-        while end < min(r + SLICE, nr) and cell_of[end] == c0:
-            end += 1
+    for c0, r, end in _cell_slices(nr, n_cells, replica_index_base, replicas_per_cell):
         part = {f: np.zeros(shape) for f in fields}
         reps = np.zeros(shape, np.int64); cnt = np.zeros(shape, np.int64); mx = np.full(shape, -np.inf)
         for q in range(r, end):
@@ -142,5 +179,26 @@ def cell_totals_reference(buckets, n_cells: int, *, replica_index_base: int = 0,
         for f in fields:
             c[f] = c[f] + part[f]
         c["max"] = np.where(mx > c["max"], mx, c["max"])
-        r = end
+    return out
+
+
+def cell_percentile_totals_reference(buckets, pct, n_cells: int, *, replica_index_base: int = 0,
+                                     replicas_per_cell: int = 1):
+    """numpy restatement of hs_read_bucket_percentile_totals over per-replica records ``buckets`` [replicas, rows, n + 1]
+    (BUCKET_DTYPE) and their percentiles ``pct`` [replicas, rows, n + 1, 2], in the device's order and slices (see
+    cell_totals_reference); a replica contributes to a bucket only if its record there has samples.  Returns
+    BUCKET_PCT_TOTAL_DTYPE [n_cells, rows, n + 1]."""
+    shape = buckets.shape[1:]
+    out = np.zeros((n_cells,) + shape, A.BUCKET_PCT_TOTAL_DTYPE)
+    for c0, r, end in _cell_slices(buckets.shape[0], n_cells, replica_index_base, replicas_per_cell):
+        part = {f: np.zeros(shape) for f in A.BUCKET_PCT_TOTAL_DTYPE.names}
+        for q in range(r, end):
+            has = buckets[q]["count"] > 0
+            for f, i in (("p50", 0), ("p99", 1)):
+                v = pct[q][..., i]
+                part[f + "_sum"] = np.where(has, part[f + "_sum"] + v, part[f + "_sum"])
+                part[f + "_sq_sum"] = np.where(has, part[f + "_sq_sum"] + v * v, part[f + "_sq_sum"])
+        c = out[c0]
+        for f in part:
+            c[f] = c[f] + part[f]
     return out

@@ -102,6 +102,9 @@ struct hs_engine {
     double last_bkt_w = 0.0; uint32_t last_bkt_n = 0;
     uint32_t bkt_rows = 0;
     dev_buf d_buckets, d_bkt_past, d_bkt_partial, d_bkt_out, d_bkt_index;
+    /* bucket percentiles (hs_set_bucket_percentiles): the sample capacity for the next runs and the last run's */
+    uint32_t bkt_cap = 0, last_bkt_cap = 0;
+    dev_buf d_bkt_vals, d_bkt_pct, d_bkt_status;
 };
 
 /* ---- validation ----------------------------------------------------------- */
@@ -353,7 +356,7 @@ static int timed_launch(hs_engine *E, const hs_launch_info &info, Kernel kern, A
 #define HS_K4(K, F) K<F>, K<F + 1>, K<F + 2>, K<F + 3>
 
 static int launch_lane(hs_engine *E, const hs_kernel_run &R, const hs_kernel_out &O, bool want_hash, bool want_rec,
-                       const hs_bucket_args &BK)
+                       const hs_bucket_pct_args &BK)
 {
     const hs_lane_model &M = E->lane_model;
     const uint32_t n = R.n_replicas;
@@ -365,21 +368,33 @@ static int launch_lane(hs_engine *E, const hs_kernel_run &R, const hs_kernel_out
                         M.svc_kind == HS_SVC_EXPONENTIAL && M.policy == HS_Q_FIFO && M.capacity < 0 &&
                         M.stop_after < 0 && M.dst_id >= 0 && M.dst_kind == HS_ENT_SINK && M.c_max == 1;
     const bool buckets = BK.n != 0;                /* never with the recorder: hs_run refuses that combination */
+    const bool pct = buckets && BK.cap != 0;
     const int fl = (want_hash ? HS_LF_HASH : 0) | (want_rec ? HS_LF_REC : 0) |
-                   (M.has_profile ? HS_LF_PROFILE : 0) | (simple ? HS_LF_SIMPLE : 0) | (buckets ? HS_LF_BUCKETS : 0);
+                   (M.has_profile ? HS_LF_PROFILE : 0) | (simple ? HS_LF_SIMPLE : 0) | (buckets ? HS_LF_BUCKETS : 0) |
+                   (pct ? HS_LF_BUCKET_PCT : 0);
     using kernel = void (*)(hs_lane_model, hs_kernel_run, hs_lane_state *, hs_ring_entry *, hs_cont *, hs_kernel_out, hs_no_bucket_args);
     using bucket_kernel = void (*)(hs_lane_model, hs_kernel_run, hs_lane_state *, hs_ring_entry *, hs_cont *, hs_kernel_out, hs_bucket_args);
+    using pct_kernel = void (*)(hs_lane_model, hs_kernel_run, hs_lane_state *, hs_ring_entry *, hs_cont *, hs_kernel_out, hs_bucket_pct_args);
     static const kernel kernels[] = {HS_K4(hs_lane_kernel, 0), HS_K4(hs_lane_kernel, 4),     /* fl <= 11: the SIMPLE */
                                      HS_K4(hs_lane_kernel, 8)};                               /* model has no profile */
     /* [HASH | PROFILE ? 2 : 0 | SIMPLE ? 4 : 0] */
     static const bucket_kernel bucket_kernels[] = {hs_lane_kernel<HS_LF_BUCKETS>, hs_lane_kernel<HS_LF_BUCKETS | HS_LF_HASH>,
                                             hs_lane_kernel<HS_LF_BUCKETS | HS_LF_PROFILE>, hs_lane_kernel<HS_LF_BUCKETS | HS_LF_PROFILE | HS_LF_HASH>,
                                             hs_lane_kernel<HS_LF_BUCKETS | HS_LF_SIMPLE>, hs_lane_kernel<HS_LF_BUCKETS | HS_LF_SIMPLE | HS_LF_HASH>};
+    /* with percentiles, the same order */
+#define HS_LP_(F) hs_lane_kernel<HS_LF_BUCKETS | HS_LF_BUCKET_PCT | (F)>
+    static const pct_kernel pct_kernels[] = {HS_LP_(0), HS_LP_(HS_LF_HASH), HS_LP_(HS_LF_PROFILE), HS_LP_(HS_LF_PROFILE | HS_LF_HASH),
+                                             HS_LP_(HS_LF_SIMPLE), HS_LP_(HS_LF_SIMPLE | HS_LF_HASH)};
+#undef HS_LP_
     const hs_launch_info info = {2, HS_KERNEL_LANE, (uint32_t)fl, 1, 0, (n + HS_LANE_THREADS - 1) / HS_LANE_THREADS,
                                  HS_LANE_THREADS, 0};
+    const uint32_t bi = (fl & HS_LF_HASH) | (M.has_profile ? 2 : 0) | (simple ? 4 : 0);
+    if (pct)
+        return timed_launch(E, info, pct_kernels[bi], M, R, (hs_lane_state *)E->d_state.p, (hs_ring_entry *)E->d_rings.p,
+                            (hs_cont *)E->d_conts.p, O, BK);
     if (buckets)
-        return timed_launch(E, info, bucket_kernels[(fl & HS_LF_HASH) | (M.has_profile ? 2 : 0) | (simple ? 4 : 0)], M, R,
-                            (hs_lane_state *)E->d_state.p, (hs_ring_entry *)E->d_rings.p, (hs_cont *)E->d_conts.p, O, BK);
+        return timed_launch(E, info, bucket_kernels[bi], M, R, (hs_lane_state *)E->d_state.p, (hs_ring_entry *)E->d_rings.p,
+                            (hs_cont *)E->d_conts.p, O, (const hs_bucket_args &)BK);
     return timed_launch(E, info, kernels[fl], M, R, (hs_lane_state *)E->d_state.p, (hs_ring_entry *)E->d_rings.p,
                         (hs_cont *)E->d_conts.p, O, hs_no_bucket_args());
 }
@@ -453,7 +468,7 @@ static int general_setup(hs_engine *E, const hs_kernel_run &R, bool thread, bool
 }
 
 static int launch_warp(hs_engine *E, const hs_kernel_run &R, const hs_kernel_out &O, bool want_hash, bool want_rec,
-                       hs_bucket_args BK)
+                       hs_bucket_pct_args BK)
 {
     hs_warp_model M;
     int fl, rc;
@@ -474,18 +489,31 @@ static int launch_warp(hs_engine *E, const hs_kernel_run &R, const hs_kernel_out
     CUDA_TRY(cudaMemsetAsync(E->d_counter.p, 0, 16, E->stream));
     using kernel = void (*)(hs_warp_model, hs_kernel_run, unsigned char *, hs_wring_entry *, hs_kernel_out, unsigned int *, hs_no_bucket_args);
     using bucket_kernel = void (*)(hs_warp_model, hs_kernel_run, unsigned char *, hs_wring_entry *, hs_kernel_out, unsigned int *, hs_bucket_args);
+    using pct_kernel = void (*)(hs_warp_model, hs_kernel_run, unsigned char *, hs_wring_entry *, hs_kernel_out, unsigned int *, hs_bucket_pct_args);
     static const kernel kernels[] = {HS_K4(hs_warp_kernel, 0), HS_K4(hs_warp_kernel, 4)};
     static const kernel fault_kernels[] = {HS_K4(hs_warp_kernel, HS_WF_FAULTS | HS_WF_PROFILE)};
     /* time buckets (never with the recorder): [HASH | FAULTS ? 2 : 0], the profile path always compiled in */
     static const bucket_kernel bucket_kernels[] = {hs_warp_kernel<HS_WF_BUCKETS | HS_WF_PROFILE>, hs_warp_kernel<HS_WF_BUCKETS | HS_WF_PROFILE | HS_WF_HASH>,
                                             hs_warp_kernel<HS_WF_BUCKETS | HS_WF_FAULTS | HS_WF_PROFILE>,
                                             hs_warp_kernel<HS_WF_BUCKETS | HS_WF_FAULTS | HS_WF_PROFILE | HS_WF_HASH>};
-    const hs_launch_info info = {1, HS_KERNEL_WARP, (uint32_t)(fl | (BK.n ? HS_WF_BUCKETS | HS_WF_PROFILE : 0)), 1, 0, grid, warps * 32, smem};
+    /* with percentiles, the same order */
+#define HS_WP_(F) hs_warp_kernel<HS_WF_BUCKETS | HS_WF_BUCKET_PCT | HS_WF_PROFILE | (F)>
+    static const pct_kernel pct_kernels[] = {HS_WP_(0), HS_WP_(HS_WF_HASH), HS_WP_(HS_WF_FAULTS), HS_WP_(HS_WF_FAULTS | HS_WF_HASH)};
+#undef HS_WP_
+    const bool pct = BK.n && BK.cap;
+    const hs_launch_info info = {1, HS_KERNEL_WARP, (uint32_t)(fl | (BK.n ? HS_WF_BUCKETS | HS_WF_PROFILE : 0) | (pct ? HS_WF_BUCKET_PCT : 0)),
+                                 1, 0, grid, warps * 32, smem};
+    const uint32_t bi = (fl & HS_WF_HASH) | ((fl & HS_WF_FAULTS) ? 2 : 0);
+    if (pct) {
+        CUDA_TRY(cudaFuncSetAttribute(pct_kernels[bi], cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
+        return timed_launch(E, info, pct_kernels[bi], M, R, (unsigned char *)E->d_state.p, (hs_wring_entry *)E->d_rings.p, O,
+                            (unsigned int *)E->d_counter.p, BK);
+    }
     if (BK.n) {
-        const bucket_kernel kern = bucket_kernels[(fl & HS_WF_HASH) | ((fl & HS_WF_FAULTS) ? 2 : 0)];
+        const bucket_kernel kern = bucket_kernels[bi];
         CUDA_TRY(cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
         return timed_launch(E, info, kern, M, R, (unsigned char *)E->d_state.p, (hs_wring_entry *)E->d_rings.p, O,
-                            (unsigned int *)E->d_counter.p, BK);
+                            (unsigned int *)E->d_counter.p, (const hs_bucket_args &)BK);
     }
     const kernel kern = (fl & HS_WF_FAULTS) ? fault_kernels[fl & 3] : kernels[fl];
     CUDA_TRY(cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
@@ -494,7 +522,7 @@ static int launch_warp(hs_engine *E, const hs_kernel_run &R, const hs_kernel_out
 }
 
 static int launch_thread(hs_engine *E, hs_kernel_run R, const hs_kernel_out &O, bool want_hash, bool want_rec, bool linked,
-                         hs_bucket_args BK)
+                         hs_bucket_pct_args BK)
 {
     hs_warp_model M;
     int fl, rc;
@@ -526,6 +554,7 @@ static int launch_thread(hs_engine *E, hs_kernel_run R, const hs_kernel_out &O, 
     const size_t dyn_smem = (size_t)(HS_T_KS * 3u + R.heap_top) * rpb * 16;
     using kernel = void (*)(hs_warp_model, hs_kernel_run, unsigned char *, hs_wring_entry *, hs_kernel_out);
     using bucket_kernel = void (*)(hs_warp_model, hs_kernel_run, unsigned char *, hs_wring_entry *, hs_kernel_out, hs_bucket_args);
+    using pct_kernel = void (*)(hs_warp_model, hs_kernel_run, unsigned char *, hs_wring_entry *, hs_kernel_out, hs_bucket_pct_args);
     static const kernel kernels[] = {HS_K4(hs_thread_kernel, 0), HS_K4(hs_thread_kernel, 4), HS_K4(hs_thread_kernel, 8),
                                      HS_K4(hs_thread_kernel, 12), HS_K4(hs_thread_kernel, 16), HS_K4(hs_thread_kernel, 20),
                                      HS_K4(hs_thread_kernel, 24), HS_K4(hs_thread_kernel, 28)};
@@ -546,24 +575,103 @@ static int launch_thread(hs_engine *E, hs_kernel_run R, const hs_kernel_out &O, 
 #define HS_TBW_(F) hs_thread_bucket_kernel_wide<HS_WF_BUCKETS | HS_WF_PROFILE | (F)>
     static const bucket_kernel bucket_wide_kernels[] = {HS_TBW_(0), HS_TBW_(HS_WF_HASH), HS_TBW_(HS_WF_FAULTS), HS_TBW_(HS_WF_FAULTS | HS_WF_HASH)};
 #undef HS_TBW_
-    if (BK.n) fl |= HS_WF_BUCKETS | HS_WF_PROFILE;
+    /* with percentiles, the same order */
+#define HS_TP_(F) hs_thread_bucket_kernel<HS_WF_BUCKETS | HS_WF_BUCKET_PCT | HS_WF_PROFILE | (F)>
+    static const pct_kernel pct_kernels[] = {HS_TP_(0), HS_TP_(HS_WF_HASH), HS_TP_(HS_WF_HEAPTOP), HS_TP_(HS_WF_HEAPTOP | HS_WF_HASH),
+                                             HS_TP_(HS_WF_FAULTS), HS_TP_(HS_WF_FAULTS | HS_WF_HASH),
+                                             HS_TP_(HS_WF_FAULTS | HS_WF_HEAPTOP), HS_TP_(HS_WF_FAULTS | HS_WF_HEAPTOP | HS_WF_HASH)};
+#undef HS_TP_
+#define HS_TPW_(F) hs_thread_bucket_kernel_wide<HS_WF_BUCKETS | HS_WF_BUCKET_PCT | HS_WF_PROFILE | (F)>
+    static const pct_kernel pct_wide_kernels[] = {HS_TPW_(0), HS_TPW_(HS_WF_HASH), HS_TPW_(HS_WF_FAULTS), HS_TPW_(HS_WF_FAULTS | HS_WF_HASH)};
+#undef HS_TPW_
+    if (BK.n) fl |= HS_WF_BUCKETS | HS_WF_PROFILE | (BK.cap ? HS_WF_BUCKET_PCT : 0);
     /* small launches (every block resident at 4 blocks per SM, no shared-memory heap top, not linked): the spill-free
      * instantiation, see hs_thread_kernel_wide */
     const bool wide = !R.heap_top && !linked && tblocks <= (uint32_t)E->sm_count * HS_T_WIDE_BLOCKS;
     if (!wide) fl |= (R.heap_top ? HS_WF_HEAPTOP : 0) | (linked ? HS_WF_LINKED : 0);
     const hs_launch_info info = {3, wide ? (uint32_t)HS_KERNEL_THREAD_WIDE : (uint32_t)HS_KERNEL_THREAD, (uint32_t)fl,
                                  R.lane_stride, R.heap_top, tblocks, HS_THREAD_BLOCK, (uint32_t)dyn_smem};
-    if (fl & HS_WF_BUCKETS) {
-        const bucket_kernel kern = wide ? bucket_wide_kernels[(fl & HS_WF_HASH) | ((fl & HS_WF_FAULTS) ? 2 : 0)]
-                                        : bucket_kernels[(fl & HS_WF_HASH) | ((fl & HS_WF_HEAPTOP) ? 2 : 0) | ((fl & HS_WF_FAULTS) ? 4 : 0)];
-        return timed_launch(E, info, kern, M, R, (unsigned char *)E->d_state.p, (hs_wring_entry *)E->d_rings.p, O, BK);
-    }
+    const uint32_t bi = (fl & HS_WF_HASH) | ((fl & HS_WF_HEAPTOP) ? 2 : 0) | ((fl & HS_WF_FAULTS) ? 4 : 0);
+    const uint32_t wbi = (fl & HS_WF_HASH) | ((fl & HS_WF_FAULTS) ? 2 : 0);
+    if (fl & HS_WF_BUCKET_PCT)
+        return timed_launch(E, info, wide ? pct_wide_kernels[wbi] : pct_kernels[bi], M, R, (unsigned char *)E->d_state.p,
+                            (hs_wring_entry *)E->d_rings.p, O, BK);
+    if (fl & HS_WF_BUCKETS)
+        return timed_launch(E, info, wide ? bucket_wide_kernels[wbi] : bucket_kernels[bi], M, R, (unsigned char *)E->d_state.p,
+                            (hs_wring_entry *)E->d_rings.p, O, (const hs_bucket_args &)BK);
     const kernel kern = !(fl & HS_WF_FAULTS) ? (wide ? wide_kernels[fl] : kernels[fl])
                       : wide ? fault_wide_kernels[fl & 3]
                       : fault_kernels[(fl & 3) | ((fl & HS_WF_HEAPTOP) ? 4 : 0) | ((fl & HS_WF_LINKED) ? 8 : 0)];
     return timed_launch(E, info, kern, M, R, (unsigned char *)E->d_state.p, (hs_wring_entry *)E->d_rings.p, O);
 }
 #undef HS_K4
+
+/* The per-cell reduction of the last run's bucket data `src` into `out` [n_cells][rows][n + 1] of T (hs_bucket_total
+ * or hs_bucket_pct_total): the two fixed-order stages of hs_buckets.cuh over the same slices. */
+template <class Src, class T>
+static int reduce_bucket_cells(hs_engine *E, const Src &src, T *out, uint32_t n_cells, const char *what)
+{
+    const hs_run_params &p = E->last;
+    const uint32_t per = E->bkt_rows * (E->last_bkt_n + 1u);
+    if (per == 0) return HS_OK;
+    CUDA_TRY(cudaSetDevice(E->device));
+    /* slices: at most HS_BUCKET_SLICE consecutive replicas of one cell (cell = (global index / replicas_per_cell) % n_cells:
+     * a plain ensemble is one cell, so its slices are 256 replicas each); per cell its slices in index order */
+    std::vector<hs_bucket_slice> slices;
+    std::vector<uint32_t> slice_cell;
+    const auto cell_of = [&](uint64_t r) { return (uint32_t)((((uint64_t)p.replica_index_base + r) / p.replicas_per_cell) % n_cells); };
+    for (uint32_t r = 0; r < p.n_replicas;) {
+        const uint32_t c = cell_of(r);
+        const uint64_t lim = std::min<uint64_t>((uint64_t)r + HS_BUCKET_SLICE, p.n_replicas);
+        uint64_t end = r;
+        while (end < lim && cell_of(end) == c) {     /* whole runs of replicas_per_cell replicas at a time */
+            const uint64_t run = ((uint64_t)p.replica_index_base + end) / p.replicas_per_cell;
+            end = std::min<uint64_t>((run + 1) * p.replicas_per_cell - p.replica_index_base, lim);
+        }
+        slices.push_back({r, (uint32_t)end});
+        slice_cell.push_back(c);
+        r = (uint32_t)end;
+    }
+    std::vector<uint32_t> first(n_cells + 1, 0), order(slices.size());
+    for (uint32_t c : slice_cell) first[c + 1]++;
+    for (uint32_t c = 0; c < n_cells; ++c) first[c + 1] += first[c];
+    {
+        std::vector<uint32_t> at(first.begin(), first.end() - 1);
+        for (uint32_t s = 0; s < (uint32_t)slices.size(); ++s) order[at[slice_cell[s]]++] = s;
+    }
+    const uint32_t ns = (uint32_t)slices.size();
+    const size_t idx_bytes = (size_t)ns * sizeof(hs_bucket_slice) + (first.size() + order.size()) * 4;
+    {
+        const double bytes = ((double)ns + n_cells) * per * sizeof(T) + (double)idx_bytes;
+        size_t free_b = 0, total_b = 0;
+        CUDA_TRY(cudaMemGetInfo(&free_b, &total_b));
+        const double have = (double)free_b + E->d_bkt_partial.n + E->d_bkt_out.n + E->d_bkt_index.n;
+        if (bytes > have)
+            return fail(HS_ERR_INVALID, "the %s cell reduction needs %.3f GB (%u slices + %u cells x %u records x %u B), the device has %.3f GB free",
+                        what, bytes / 1e9, ns, n_cells, per, (uint32_t)sizeof(T), have / 1e9);
+    }
+    int rc;
+    if ((rc = E->d_bkt_index.ensure(idx_bytes))) return rc;
+    if ((rc = E->d_bkt_partial.ensure((size_t)ns * per * sizeof(T)))) return rc;
+    if ((rc = E->d_bkt_out.ensure((size_t)n_cells * per * sizeof(T)))) return rc;
+    unsigned char *ix = (unsigned char *)E->d_bkt_index.p;
+    const hs_bucket_slice *d_slices = (const hs_bucket_slice *)ix;
+    const uint32_t *d_first = (const uint32_t *)(ix + (size_t)ns * sizeof(hs_bucket_slice));
+    const uint32_t *d_order = d_first + first.size();
+    CUDA_TRY(cudaMemcpyAsync(ix, slices.data(), (size_t)ns * sizeof(hs_bucket_slice), cudaMemcpyHostToDevice, E->stream));
+    CUDA_TRY(cudaMemcpyAsync((void *)d_first, first.data(), first.size() * 4, cudaMemcpyHostToDevice, E->stream));
+    CUDA_TRY(cudaMemcpyAsync((void *)d_order, order.data(), order.size() * 4, cudaMemcpyHostToDevice, E->stream));
+    const dim3 g1((per + 127) / 128, std::min<uint32_t>(ns, 65535u)), g2((per + 127) / 128, std::min<uint32_t>(n_cells, 65535u));
+    hs_bucket_partial_kernel<Src, T><<<g1, 128, 0, E->stream>>>(src, per, d_slices, ns, (T *)E->d_bkt_partial.p);
+    CUDA_TRY(cudaGetLastError());
+    hs_bucket_final_kernel<T><<<g2, 128, 0, E->stream>>>((const T *)E->d_bkt_partial.p, per, d_first, d_order, n_cells,
+                                                         (T *)E->d_bkt_out.p);
+    CUDA_TRY(cudaGetLastError());
+    E->launches += 2;
+    CUDA_TRY(cudaMemcpyAsync(out, E->d_bkt_out.p, (size_t)n_cells * per * sizeof(T), cudaMemcpyDeviceToHost, E->stream));
+    CUDA_TRY(cudaStreamSynchronize(E->stream));   /* the host vectors above are the copies' sources */
+    return HS_OK;
+}
 
 /* ---- entry points ------------------------------------------------------- */
 
@@ -614,7 +722,8 @@ int hs_engine_destroy(hs_engine *E)
                        &E->d_srv_index, &E->d_counter, &E->d_trace_arr, &E->d_trace_svc, &E->d_profiles, &E->d_profile_table, &E->d_hist, &E->d_cell_totals, &E->d_conts,
                        &E->d_sketch_tab, &E->d_sketch, &E->d_sketch_merged, &E->d_key_cdf,
                        &E->d_outbox, &E->d_outbox_n, &E->d_inbox, &E->d_inbox_n,
-                       &E->d_buckets, &E->d_bkt_past, &E->d_bkt_partial, &E->d_bkt_out, &E->d_bkt_index};
+                       &E->d_buckets, &E->d_bkt_past, &E->d_bkt_partial, &E->d_bkt_out, &E->d_bkt_index,
+                       &E->d_bkt_vals, &E->d_bkt_pct, &E->d_bkt_status};
     for (dev_buf *b : bufs) b->release();
     if (E->ev0) cudaEventDestroy(E->ev0);
     if (E->ev1) cudaEventDestroy(E->ev1);
@@ -740,6 +849,8 @@ int hs_run(hs_engine *E, const hs_run_params *p)
     if (engine == 2 && faults) return fail(HS_ERR_INVALID, "the lane engine does not run fault schedules (the model has FAULT rows): use engine 0, 1 or 3");
     if (engine == 2 && !E->lane_ok) return fail(HS_ERR_INVALID, "lane engine needs Source -> Server(concurrency <= 64) -> Sink|Counter");
 
+    if (E->bkt_cap && !E->bkt_n)
+        return fail(HS_ERR_INVALID, "bucket percentiles need time buckets (hs_set_buckets with n > 0)");
     const uint32_t ring = p->queue_ring ? pow2_at_least(p->queue_ring) : engine == 2 ? 256 : 128;
     const bool want_hist = (p->flags & HS_RUN_HISTOGRAM) != 0;
     if (p->resume) {
@@ -754,12 +865,16 @@ int hs_run(hs_engine *E, const hs_run_params *p)
         if (want_hist != E->hist_on) return fail(HS_ERR_STATE, "resume must keep HS_RUN_HISTOGRAM");
         if (E->bkt_n != E->last_bkt_n || (E->bkt_n && E->bkt_w != E->last_bkt_w))
             return fail(HS_ERR_STATE, "resume must keep the bucket configuration of the paused run (hs_set_buckets)");
+        if (E->bkt_cap != E->last_bkt_cap)
+            return fail(HS_ERR_STATE, "resume must keep the bucket sample capacity of the paused run (hs_set_bucket_percentiles: %u, paused with %u)",
+                        E->bkt_cap, E->last_bkt_cap);
         if (ring != E->last_ring) return fail(HS_ERR_STATE, "resume must keep queue_ring");
     }
 
     const uint32_t n = p->n_replicas;
     const uint32_t ne = (uint32_t)E->ents.size();
     const size_t bkt_records = E->bkt_n ? (size_t)n * E->bkt_rows * ((size_t)E->bkt_n + 1) : 0;
+    const size_t bkt_vals = bkt_records && E->bkt_cap ? (size_t)n * E->bkt_rows * E->bkt_cap : 0;     /* percentile value buffers */
     if (E->bkt_n) {
         if (linked) return fail(HS_ERR_INVALID, "time buckets are not available on the windows of a linked partition");
         if (p->record_cap || p->sample_cap || p->service_cap)
@@ -769,12 +884,16 @@ int hs_run(hs_engine *E, const hs_run_params *p)
         if (!(last < (double)E->bkt_n))
             return fail(HS_ERR_INVALID, "%u buckets of %g s end before the end time %.9f s (bucket %.0f): n * width must exceed it",
                         E->bkt_n, E->bkt_w, hs_ns_to_seconds(p->end_ns), last);
-        const double bytes = (double)n * E->bkt_rows * ((double)E->bkt_n + 1) * sizeof(hs_bucket) + (double)n * E->bkt_rows * 8.0;
+        /* records (32 B, and 16 B of percentiles with hs_set_bucket_percentiles), past-end indices, value buffers */
+        const uint32_t rec_b = (uint32_t)sizeof(hs_bucket) + (E->bkt_cap ? 2u * (uint32_t)sizeof(double) : 0u);
+        const double bytes = (double)n * E->bkt_rows * ((double)E->bkt_n + 1) * rec_b + (double)n * E->bkt_rows * 8.0 +
+                             (double)n * E->bkt_rows * E->bkt_cap * 8.0 + (E->bkt_cap ? (double)n * 4.0 : 0.0);
         size_t free_b = 0, total_b = 0;
         CUDA_TRY(cudaMemGetInfo(&free_b, &total_b));
-        if (bytes > (double)(free_b + E->d_buckets.n + E->d_bkt_past.n))
-            return fail(HS_ERR_INVALID, "time buckets need %.3f GB (%u replicas x %u rows x %u buckets x 32 B), the device has %.3f GB free",
-                        bytes / 1e9, n, E->bkt_rows, E->bkt_n + 1, (double)(free_b + E->d_buckets.n + E->d_bkt_past.n) / 1e9);
+        const double have = (double)(free_b + E->d_buckets.n + E->d_bkt_past.n + E->d_bkt_vals.n + E->d_bkt_pct.n + E->d_bkt_status.n);
+        if (bytes > have)
+            return fail(HS_ERR_INVALID, "time buckets need %.3f GB (%u replicas x %u rows x %u buckets x %u B, %u percentile samples x 8 B "
+                        "per row), the device has %.3f GB free", bytes / 1e9, n, E->bkt_rows, E->bkt_n + 1, rec_b, E->bkt_cap, have / 1e9);
     }
     int rc;
     if (bkt_records) {
@@ -783,6 +902,15 @@ int hs_run(hs_engine *E, const hs_run_params *p)
         if (!p->resume) {
             CUDA_TRY(cudaMemsetAsync(E->d_buckets.p, 0, bkt_records * sizeof(hs_bucket), E->stream));
             CUDA_TRY(cudaMemsetAsync(E->d_bkt_past.p, 0, (size_t)n * E->bkt_rows * 8, E->stream));
+        }
+    }
+    if (bkt_vals) {                                  /* the buffers need no clearing: a bucket reads only what it stored */
+        if ((rc = E->d_bkt_vals.ensure(bkt_vals * sizeof(double)))) return rc;
+        if ((rc = E->d_bkt_pct.ensure(bkt_records * 2 * sizeof(double)))) return rc;
+        if ((rc = E->d_bkt_status.ensure((size_t)n * 4))) return rc;
+        if (!p->resume) {
+            CUDA_TRY(cudaMemsetAsync(E->d_bkt_pct.p, 0, bkt_records * 2 * sizeof(double), E->stream));
+            CUDA_TRY(cudaMemsetAsync(E->d_bkt_status.p, 0, (size_t)n * 4, E->stream));
         }
     }
     if ((rc = E->d_summ.ensure((size_t)n * sizeof(hs_replica_summary)))) return rc;
@@ -837,10 +965,14 @@ int hs_run(hs_engine *E, const hs_run_params *p)
     O.sketch = (uint8_t *)E->d_sketch.p;
     O.outbox = (hs_xevent *)E->d_outbox.p; O.outbox_n = (uint32_t *)E->d_outbox_n.p;
     O.inbox = (hs_xevent *)E->d_inbox.p; O.inbox_n = (uint32_t *)E->d_inbox_n.p;
-    hs_bucket_args BK;
+    hs_bucket_pct_args BK;
     BK.w = E->bkt_w; BK.n = E->bkt_n; BK.rows = E->bkt_rows; BK.acc_off = 0; BK.pad = 0;
     BK.rec = bkt_records ? (hs_bucket *)E->d_buckets.p : nullptr;
     BK.past_end = bkt_records ? (int64_t *)E->d_bkt_past.p : nullptr;
+    BK.cap = bkt_vals ? E->bkt_cap : 0u; BK.pad2 = 0;      /* cap = 0: no percentiles, the launchers pass hs_bucket_args */
+    BK.vals = bkt_vals ? (double *)E->d_bkt_vals.p : nullptr;
+    BK.pct = bkt_vals ? (double2 *)E->d_bkt_pct.p : nullptr;
+    BK.status = bkt_vals ? (uint32_t *)E->d_bkt_status.p : nullptr;
     const bool want_hash = (p->flags & HS_RUN_ORDER_HASH) != 0;
     const bool want_rec = (p->record_cap | p->sample_cap | p->service_cap) != 0;
     rc = engine == 2 ? launch_lane(E, R, O, want_hash, want_rec, BK)
@@ -848,7 +980,7 @@ int hs_run(hs_engine *E, const hs_run_params *p)
        : launch_warp(E, R, O, want_hash, want_rec, BK);
     if (rc) return rc;
     E->last = *p;
-    E->last_bkt_w = E->bkt_w; E->last_bkt_n = E->bkt_n;
+    E->last_bkt_w = E->bkt_w; E->last_bkt_n = E->bkt_n; E->last_bkt_cap = E->bkt_cap;
     E->last_engine = engine;
     E->last_ring = ring;
     E->have_run = true;
@@ -907,66 +1039,40 @@ int hs_read_bucket_totals(hs_engine *E, hs_bucket_total *out, uint32_t n_cells)
     if (!E || !out || n_cells == 0) return fail(HS_ERR_INVALID, "bad argument");
     if (!E->have_run) return fail(HS_ERR_STATE, "no run yet");
     if (!E->last_bkt_n) return fail(HS_ERR_STATE, "the last run had no time buckets (hs_set_buckets)");
-    const hs_run_params &p = E->last;
-    const uint32_t per = E->bkt_rows * (E->last_bkt_n + 1u);
-    if (per == 0) return HS_OK;
-    CUDA_TRY(cudaSetDevice(E->device));
-    /* slices: at most HS_BUCKET_SLICE consecutive replicas of one cell (cell = (global index / replicas_per_cell) % n_cells:
-     * a plain ensemble is one cell, so its slices are 256 replicas each); per cell its slices in index order */
-    std::vector<hs_bucket_slice> slices;
-    std::vector<uint32_t> slice_cell;
-    const auto cell_of = [&](uint64_t r) { return (uint32_t)((((uint64_t)p.replica_index_base + r) / p.replicas_per_cell) % n_cells); };
-    for (uint32_t r = 0; r < p.n_replicas;) {
-        const uint32_t c = cell_of(r);
-        const uint64_t lim = std::min<uint64_t>((uint64_t)r + HS_BUCKET_SLICE, p.n_replicas);
-        uint64_t end = r;
-        while (end < lim && cell_of(end) == c) {     /* whole runs of replicas_per_cell replicas at a time */
-            const uint64_t run = ((uint64_t)p.replica_index_base + end) / p.replicas_per_cell;
-            end = std::min<uint64_t>((run + 1) * p.replicas_per_cell - p.replica_index_base, lim);
-        }
-        slices.push_back({r, (uint32_t)end});
-        slice_cell.push_back(c);
-        r = (uint32_t)end;
-    }
-    std::vector<uint32_t> first(n_cells + 1, 0), order(slices.size());
-    for (uint32_t c : slice_cell) first[c + 1]++;
-    for (uint32_t c = 0; c < n_cells; ++c) first[c + 1] += first[c];
-    {
-        std::vector<uint32_t> at(first.begin(), first.end() - 1);
-        for (uint32_t s = 0; s < (uint32_t)slices.size(); ++s) order[at[slice_cell[s]]++] = s;
-    }
-    const uint32_t ns = (uint32_t)slices.size();
-    const size_t idx_bytes = (size_t)ns * sizeof(hs_bucket_slice) + (first.size() + order.size()) * 4;
-    {
-        const double bytes = ((double)ns + n_cells) * per * sizeof(hs_bucket_total) + (double)idx_bytes;
-        size_t free_b = 0, total_b = 0;
-        CUDA_TRY(cudaMemGetInfo(&free_b, &total_b));
-        const double have = (double)free_b + E->d_bkt_partial.n + E->d_bkt_out.n + E->d_bkt_index.n;
-        if (bytes > have)
-            return fail(HS_ERR_INVALID, "the bucket cell reduction needs %.3f GB (%u slices + %u cells x %u records x 48 B), the device has %.3f GB free",
-                        bytes / 1e9, ns, n_cells, per, have / 1e9);
-    }
-    int rc;
-    if ((rc = E->d_bkt_index.ensure(idx_bytes))) return rc;
-    if ((rc = E->d_bkt_partial.ensure((size_t)ns * per * sizeof(hs_bucket_total)))) return rc;
-    if ((rc = E->d_bkt_out.ensure((size_t)n_cells * per * sizeof(hs_bucket_total)))) return rc;
-    unsigned char *ix = (unsigned char *)E->d_bkt_index.p;
-    const hs_bucket_slice *d_slices = (const hs_bucket_slice *)ix;
-    const uint32_t *d_first = (const uint32_t *)(ix + (size_t)ns * sizeof(hs_bucket_slice));
-    const uint32_t *d_order = d_first + first.size();
-    CUDA_TRY(cudaMemcpyAsync(ix, slices.data(), (size_t)ns * sizeof(hs_bucket_slice), cudaMemcpyHostToDevice, E->stream));
-    CUDA_TRY(cudaMemcpyAsync((void *)d_first, first.data(), first.size() * 4, cudaMemcpyHostToDevice, E->stream));
-    CUDA_TRY(cudaMemcpyAsync((void *)d_order, order.data(), order.size() * 4, cudaMemcpyHostToDevice, E->stream));
-    const dim3 g1((per + 127) / 128, std::min<uint32_t>(ns, 65535u)), g2((per + 127) / 128, std::min<uint32_t>(n_cells, 65535u));
-    hs_bucket_partial_kernel<<<g1, 128, 0, E->stream>>>((const hs_bucket *)E->d_buckets.p, per, d_slices, ns, (hs_bucket_total *)E->d_bkt_partial.p);
-    CUDA_TRY(cudaGetLastError());
-    hs_bucket_final_kernel<<<g2, 128, 0, E->stream>>>((const hs_bucket_total *)E->d_bkt_partial.p, per, d_first, d_order, n_cells,
-                                                      (hs_bucket_total *)E->d_bkt_out.p);
-    CUDA_TRY(cudaGetLastError());
-    E->launches += 2;
-    CUDA_TRY(cudaMemcpyAsync(out, E->d_bkt_out.p, (size_t)n_cells * per * sizeof(hs_bucket_total), cudaMemcpyDeviceToHost, E->stream));
-    CUDA_TRY(cudaStreamSynchronize(E->stream));   /* the host vectors above are the copies' sources */
+    hs_bucket_src src;
+    src.b = (const hs_bucket *)E->d_buckets.p;
+    return reduce_bucket_cells(E, src, out, n_cells, "bucket");
+}
+
+int hs_set_bucket_percentiles(hs_engine *E, uint32_t sample_cap)
+{
+    if (!E) return fail(HS_ERR_INVALID, "engine is NULL");
+    if (sample_cap > (1u << 24)) return fail(HS_ERR_INVALID, "at most 2^24 percentile samples per bucket, got %u", sample_cap);
+    E->bkt_cap = sample_cap;
     return HS_OK;
+}
+
+int hs_read_bucket_percentiles(hs_engine *E, double *out)
+{
+    if (!E || !out) return fail(HS_ERR_INVALID, "bad argument");
+    if (!E->have_run) return fail(HS_ERR_STATE, "no run yet");
+    if (!E->last_bkt_n || !E->last_bkt_cap) return fail(HS_ERR_STATE, "the last run had no bucket percentiles (hs_set_bucket_percentiles)");
+    CUDA_TRY(cudaSetDevice(E->device));
+    const size_t nr = (size_t)E->last.n_replicas * E->bkt_rows * (E->last_bkt_n + 1u);
+    if (nr) CUDA_TRY(cudaMemcpyAsync(out, E->d_bkt_pct.p, nr * 2 * sizeof(double), cudaMemcpyDeviceToHost, E->stream));
+    CUDA_TRY(cudaStreamSynchronize(E->stream));
+    return HS_OK;
+}
+
+int hs_read_bucket_percentile_totals(hs_engine *E, hs_bucket_pct_total *out, uint32_t n_cells)
+{
+    if (!E || !out || n_cells == 0) return fail(HS_ERR_INVALID, "bad argument");
+    if (!E->have_run) return fail(HS_ERR_STATE, "no run yet");
+    if (!E->last_bkt_n || !E->last_bkt_cap) return fail(HS_ERR_STATE, "the last run had no bucket percentiles (hs_set_bucket_percentiles)");
+    hs_bucket_pct_src src;
+    src.b = (const hs_bucket *)E->d_buckets.p;
+    src.pct = (const double2 *)E->d_bkt_pct.p;
+    return reduce_bucket_cells(E, src, out, n_cells, "bucket percentile");
 }
 
 int hs_sync(hs_engine *E)

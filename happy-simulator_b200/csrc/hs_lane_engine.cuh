@@ -80,6 +80,7 @@
                              unbounded queue, Sink downstream, Philox draws -- the BASELINE configs[0]/[1] shape */
 #define HS_LF_BUCKETS 16  /* time buckets of the Sink samples (hs_set_buckets; the Sink is bucketed row 0); compiled
                              without HS_LF_REC only */
+#define HS_LF_BUCKET_PCT 32 /* with HS_LF_BUCKETS: the buckets' p50 / p99 (hs_set_bucket_percentiles) */
 
 struct hs_now_ev {        /* an event created at the current timestamp       */
     uint64_t idx;         /* Event._sort_index                               */
@@ -154,7 +155,7 @@ template <int FLAGS>
 __global__ void __launch_bounds__(HS_LANE_THREADS, 7)
 hs_lane_kernel(hs_lane_model M, hs_kernel_run P, hs_lane_state *__restrict__ states,
                hs_ring_entry *__restrict__ rings, hs_cont *__restrict__ conts, hs_kernel_out O,
-               typename hs_bucket_args_of<(FLAGS & HS_LF_BUCKETS) != 0>::type BK)
+               typename hs_bucket_args_of<(FLAGS & HS_LF_BUCKETS) != 0, (FLAGS & HS_LF_BUCKET_PCT) != 0>::type BK)
 {
     constexpr uint32_t HS_DRAW_BUF = (FLAGS & HS_LF_REC) ? HS_DRAW_BUF_RECORD : HS_DRAW_BUF_SUMMARY;
     constexpr uint32_t STAGE_ROWS = (FLAGS & HS_LF_REC) ? HS_STAGE : 1;
@@ -851,6 +852,7 @@ hs_lane_kernel(hs_lane_model M, hs_kernel_run P, hs_lane_state *__restrict__ sta
     if (!valid) return;
     if (P.resume && S->done) return;        /* finished in an earlier window: outputs already final */
     if (FLAGS & HS_LF_BUCKETS) hs_bucket_flush(BK, r, 0u, bacc);   /* the current time bucket, at the run's end or a pause */
+    if (FLAGS & HS_LF_BUCKET_PCT) status |= hs_bucket_status(BK, r);
     if ((FLAGS & HS_LF_REC) && staged) {    /* drain what is still staged, record by record */
         while (st_fl != st_wr) {
             __stcs((uint4 *)(rec + rec_pos), sh_rec[st_fl % HS_STAGE][tid]);

@@ -82,7 +82,7 @@ template <int FLAGS>
 __device__ __forceinline__ void
 hs_thread_body(const hs_warp_model &M, const hs_kernel_run &P, unsigned char *__restrict__ blocks,
                hs_wring_entry *__restrict__ rings, const hs_kernel_out &O,
-               const typename hs_bucket_args_of<(FLAGS & HS_WF_BUCKETS) != 0>::type BK)
+               const typename hs_bucket_args_of<(FLAGS & HS_WF_BUCKETS) != 0, (FLAGS & HS_WF_BUCKET_PCT) != 0>::type BK)
 {
     /* dynamic shared memory of a block: [ now tier: HS_T_KS x 3 chunks x rpb columns | heap top: P.heap_top keys x rpb columns ],
      * rpb = replicas (columns) of the block.  The now tier is sized by the columns in use (it was 64 wide whatever the
@@ -802,6 +802,7 @@ hs_thread_body(const hs_warp_model &M, const hs_kernel_run &P, unsigned char *__
     hdr.done = paused ? 0 : 1;
     *Hg = hdr;
     hs_bucket_end(BK, r, bacc);                          /* every row's current time bucket, at the run's end or a pause */
+    if (FLAGS & HS_WF_BUCKET_PCT) hdr.status |= hs_bucket_status(BK, r);
     if (O.summaries) {
         hs_replica_summary s;
         s.events_processed = h_processed; s.final_time_ns = h_now;
@@ -838,11 +839,12 @@ hs_thread_kernel_wide(hs_warp_model M, hs_kernel_run P, unsigned char *__restric
 }
 
 /* the same two entry points for the time-bucket instantiations (FLAGS with HS_WF_BUCKETS): the bucket arguments come
- * as one more parameter, which the kernels above do not have */
+ * as one more parameter, which the kernels above do not have (hs_bucket_pct_args with HS_WF_BUCKET_PCT) */
 template <int FLAGS>
 __global__ void __launch_bounds__(HS_THREAD_BLOCK, HS_T_MINBLOCKS)
 hs_thread_bucket_kernel(hs_warp_model M, hs_kernel_run P, unsigned char *__restrict__ blocks,
-                        hs_wring_entry *__restrict__ rings, hs_kernel_out O, hs_bucket_args BK)
+                        hs_wring_entry *__restrict__ rings, hs_kernel_out O,
+                        typename hs_bucket_args_of<true, (FLAGS & HS_WF_BUCKET_PCT) != 0>::type BK)
 {
     hs_thread_body<FLAGS>(M, P, blocks, rings, O, BK);
 }
@@ -850,7 +852,8 @@ hs_thread_bucket_kernel(hs_warp_model M, hs_kernel_run P, unsigned char *__restr
 template <int FLAGS>
 __global__ void __launch_bounds__(HS_THREAD_BLOCK, HS_T_WIDE_BLOCKS)
 hs_thread_bucket_kernel_wide(hs_warp_model M, hs_kernel_run P, unsigned char *__restrict__ blocks,
-                             hs_wring_entry *__restrict__ rings, hs_kernel_out O, hs_bucket_args BK)
+                             hs_wring_entry *__restrict__ rings, hs_kernel_out O,
+                             typename hs_bucket_args_of<true, (FLAGS & HS_WF_BUCKET_PCT) != 0>::type BK)
 {
     hs_thread_body<FLAGS>(M, P, blocks, rings, O, BK);
 }

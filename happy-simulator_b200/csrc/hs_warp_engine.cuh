@@ -44,6 +44,7 @@
                               the tie test; compiled out of every other launch */
 #define HS_WF_BUCKETS 64   /* time buckets of the Sink / Probe samples (hs_set_buckets, hs_buckets.cuh); compiled out of every
                               other launch.  The row of a SINK / PROBE entity is the low word of its device row's d1 */
+#define HS_WF_BUCKET_PCT 128 /* with HS_WF_BUCKETS: the buckets' p50 / p99 (hs_set_bucket_percentiles) */
 
 struct __align__(16) hs_warp_hdr {      /* 128 B */
     int64_t now; uint64_t ctr; int64_t processed; uint64_t hash;
@@ -212,7 +213,7 @@ template <int FLAGS>
 __global__ void __launch_bounds__(256)
 hs_warp_kernel(hs_warp_model M, hs_kernel_run P, unsigned char *__restrict__ blocks,
                hs_wring_entry *__restrict__ rings, hs_kernel_out O, unsigned int *__restrict__ next_replica,
-               typename hs_bucket_args_of<(FLAGS & HS_WF_BUCKETS) != 0>::type BK)
+               typename hs_bucket_args_of<(FLAGS & HS_WF_BUCKETS) != 0, (FLAGS & HS_WF_BUCKET_PCT) != 0>::type BK)
 {
     extern __shared__ __align__(16) unsigned char smem_raw[];
     const int lane = threadIdx.x & 31;
@@ -460,6 +461,7 @@ hs_warp_kernel(hs_warp_model M, hs_kernel_run P, unsigned char *__restrict__ blo
         /* ---- publish + write the block back -------------------------------- */
         if (lane == 0) {
             hs_bucket_end(BK, r, bacc);                 /* every row's current time bucket, at the run's end or a pause */
+            if (FLAGS & HS_WF_BUCKET_PCT) H->status |= hs_bucket_status(BK, r);
             H->done = paused ? 0 : 1;
             if (O.summaries) {
                 hs_replica_summary s;

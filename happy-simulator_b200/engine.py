@@ -31,7 +31,8 @@ EXPORTED_SYMBOLS = ["hs_version", "hs_last_error", "hs_engine_create", "hs_engin
                     "hs_sketch_layout", "hs_read_sketches", "hs_coordinator_create", "hs_coordinator_destroy",
                     "hs_coordinator_exchange", "hs_coordinator_read", "hs_read_outbox", "hs_read_inbox",
                     "hs_partition_upload", "hs_partition_validate", "hs_set_buckets", "hs_read_buckets",
-                    "hs_read_bucket_totals"]
+                    "hs_read_bucket_totals", "hs_set_bucket_percentiles", "hs_read_bucket_percentiles",
+                    "hs_read_bucket_percentile_totals"]
 
 
 def load_library(path: str | None = None):
@@ -81,6 +82,9 @@ def load_library(path: str | None = None):
         "hs_set_buckets": ([H, C.c_double, C.c_uint32], C.c_int),
         "hs_read_buckets": ([H, C.c_void_p, C.c_void_p, C.POINTER(C.c_uint32)], C.c_int),
         "hs_read_bucket_totals": ([H, C.c_void_p, C.c_uint32], C.c_int),
+        "hs_set_bucket_percentiles": ([H, C.c_uint32], C.c_int),
+        "hs_read_bucket_percentiles": ([H, C.c_void_p], C.c_int),
+        "hs_read_bucket_percentile_totals": ([H, C.c_void_p, C.c_uint32], C.c_int),
     }
     for name, (args, res) in sigs.items():
         fn = getattr(L, name)
@@ -213,6 +217,27 @@ class Engine:
         """BUCKET_TOTAL_DTYPE [n_cells, rows, n + 1]: the last run's buckets reduced per sweep cell (hs_read_bucket_totals)."""
         out = np.zeros((n_cells, rows, n + 1), A.BUCKET_TOTAL_DTYPE)
         _check(self._L, self._L.hs_read_bucket_totals(self._h, out.ctypes.data, n_cells))
+        return out
+
+    def set_bucket_percentiles(self, sample_cap: int = 0) -> None:
+        """hs_set_bucket_percentiles: p50 / p99 of every time bucket, from at most sample_cap values per bucket, for the
+        following runs (0: off)."""
+        _check(self._L, self._L.hs_set_bucket_percentiles(self._h, int(sample_cap)))
+
+    def read_bucket_percentiles(self, n: int):
+        """float64 [n_replicas, rows, n + 1, 2]: {p50, p99} of every bucket of the last run, which had n buckets per row
+        (hs_read_bucket_percentiles; NaN where a bucket overflowed its sample capacity, 0 where it is empty)."""
+        rows = C.c_uint32()
+        _check(self._L, self._L.hs_read_buckets(self._h, None, None, C.byref(rows)))
+        out = np.zeros((int(self._params.n_replicas), int(rows.value), n + 1, 2), np.float64)
+        _check(self._L, self._L.hs_read_bucket_percentiles(self._h, out.ctypes.data))
+        return out
+
+    def read_bucket_percentile_totals(self, n_cells: int, rows: int, n: int):
+        """BUCKET_PCT_TOTAL_DTYPE [n_cells, rows, n + 1]: the last run's bucket percentiles reduced per sweep cell
+        (hs_read_bucket_percentile_totals)."""
+        out = np.zeros((n_cells, rows, n + 1), A.BUCKET_PCT_TOTAL_DTYPE)
+        _check(self._L, self._L.hs_read_bucket_percentile_totals(self._h, out.ctypes.data, n_cells))
         return out
 
     def read_box(self, which: str = "outbox"):

@@ -261,6 +261,8 @@ typedef struct hs_run_params {
                                      the other's from the run's or from the sending partition's):
                                      heapq orders such a pair by its array layout, the engines by their own heap's, so this
                                      replica's event order may differ from the reference's                               */
+#define HS_ST_BUCKET_OVERFLOW 512u /* bucket percentiles (hs_set_bucket_percentiles): a bucket held more samples than the
+                                     sample capacity; its p50 / p99 are NaN, its record's count is exact             */
 
 typedef struct hs_replica_summary {
     int64_t events_processed;  /* SimulationSummary.total_events_processed (simulation.py:553) */
@@ -359,6 +361,14 @@ typedef struct hs_bucket_total {
     double mean_sum, mean_sq_sum;  /* sum of their bucket means (sum / count) and of the squared means        */
     double max;                    /* max of their maxes (-inf if replicas == 0)                              */
 } hs_bucket_total;
+
+/* The p50 / p99 of one bucket of one row over the replicas of one sweep cell, 32 bytes, in the order and the slices
+ * of hs_bucket_total.  Only replicas with at least one sample in the bucket contribute: their number is that
+ * hs_bucket_total's `replicas`. */
+typedef struct hs_bucket_pct_total {
+    double p50_sum, p50_sq_sum;    /* sum of their bucket p50s and of the squared p50s                         */
+    double p99_sum, p99_sq_sum;    /* the same for p99                                                         */
+} hs_bucket_pct_total;
 
 /* ---- entry points ------------------------------------------------------ */
 
@@ -523,6 +533,24 @@ int hs_read_buckets(hs_engine *e, hs_bucket *out, int64_t *past_end, uint32_t *r
  * hs_read_cell_totals) on the device and copy out[n_cells][rows][n + 1] to the host.  Slot n aggregates the
  * past-end samples whatever their index. */
 int hs_read_bucket_totals(hs_engine *e, hs_bucket_total *out, uint32_t n_cells);
+
+/* Bucket percentiles for the following hs_run calls (sample_cap = 0: off, the default): besides its hs_bucket record
+ * every bucket gets the reference's _percentile_sorted(sorted(values), 0.50) and (..., 0.99)
+ * (instrumentation/data.py:197-210), bit for bit.  The engine holds the values of each row's current bucket, at most
+ * sample_cap of them per row and replica, and selects the two order-statistic pairs when the row moves on and when a
+ * launch ends.  A bucket with more than sample_cap samples gets NaN for both and sets HS_ST_BUCKET_OVERFLOW in its
+ * replica's status; its record's count says what capacity a re-run needs.  hs_run refuses percentiles without
+ * buckets (hs_set_buckets n > 0) and a resume whose capacity differs from the paused run's; its memory check covers
+ * the value buffers and the percentile records. */
+int hs_set_bucket_percentiles(hs_engine *e, uint32_t sample_cap);
+
+/* Copy the last run's bucket percentiles: out[n_replicas][rows][n + 1][2], {p50, p99} per slot as hs_read_buckets
+ * lays out the records (0, 0 for an empty bucket). */
+int hs_read_bucket_percentiles(hs_engine *e, double *out);
+
+/* Reduce the last run's bucket percentiles per sweep cell, as hs_read_bucket_totals reduces the records, and copy
+ * out[n_cells][rows][n + 1] to the host. */
+int hs_read_bucket_percentile_totals(hs_engine *e, hs_bucket_pct_total *out, uint32_t n_cells);
 
 /* Device pointer/size of the last run's totals (for the NCCL allreduce done by
  * the host layer on torch.distributed; layout = hs_totals). */
