@@ -863,17 +863,7 @@ class Simulation:
                                               f"bucket_sample_cap={cap}; pass bucket_sample_cap={need}"
                                               + (" (or more: later windows may need it)" if we >= 0 else ""), st.copy())
             if spec and we < 0:
-                w, nb = spec
-                out["buckets"], out["bucket_past_end"] = eng.read_buckets(nb)
-                n_cells = max(1, int(self.model.n_cells))
-                out["bucket_totals"] = eng.read_bucket_totals(n_cells, out["buckets"].shape[1], nb)
-                out["bucket_width_s"], out["bucket_count"] = w, nb
-                out["bucket_rows"] = _buckets.rows(self.model)
-                out["bucket_objects"] = _buckets.row_objects(self.model, self.objects)
-                if cap:
-                    out["bucket_percentiles"] = eng.read_bucket_percentiles(nb)
-                    out["bucket_percentile_totals"] = eng.read_bucket_percentile_totals(n_cells, out["buckets"].shape[1], nb)
-                    out["bucket_sample_cap"] = cap
+                out.update(_buckets.read_outputs(eng, spec, cap, self.model, self.objects, max(1, int(self.model.n_cells))))
         finally:
             eng.set_bucket_percentiles(0)       # the engine is shared: other runs get no buckets unless they ask
             eng.set_buckets(0.0, 0)

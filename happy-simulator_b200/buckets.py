@@ -81,6 +81,27 @@ def row_objects(model, objects) -> list:
     return [objects[i] if int(k[i]) == A.HS_ENT_SINK else probe_of.get(i) for i in rows(model)]
 
 
+def read_outputs(eng, spec, cap: int, model, objects, n_cells: int = 1) -> dict:
+    """The bucket keys of a bucketed ensemble's output dict, read from the engine ``eng`` after the run's last launch:
+    ``buckets`` and ``bucket_past_end`` (the records), ``bucket_totals`` (``n_cells`` cells), ``bucket_width_s``,
+    ``bucket_count``, ``bucket_rows`` and ``bucket_objects`` (the rows of ``model``, whose entity ids index
+    ``objects``), and with percentiles (``cap`` > 0) ``bucket_percentiles``, ``bucket_percentile_totals`` and
+    ``bucket_sample_cap``.  ``Simulation.run_ensemble`` and a linked run's partitions both fill their outputs here."""
+    w, nb = spec
+    out = {}
+    out["buckets"], out["bucket_past_end"] = eng.read_buckets(nb)
+    nr = out["buckets"].shape[1]
+    out["bucket_totals"] = eng.read_bucket_totals(n_cells, nr, nb)
+    out["bucket_width_s"], out["bucket_count"] = w, nb
+    out["bucket_rows"] = rows(model)
+    out["bucket_objects"] = row_objects(model, objects)
+    if cap:
+        out["bucket_percentiles"] = eng.read_bucket_percentiles(nb)
+        out["bucket_percentile_totals"] = eng.read_bucket_percentile_totals(n_cells, nr, nb)
+        out["bucket_sample_cap"] = cap
+    return out
+
+
 def _row_of(out, obj) -> int:
     for b, o in enumerate(out["bucket_objects"]):
         if o is obj or (o is not None and getattr(o, "data_sink", None) is obj):

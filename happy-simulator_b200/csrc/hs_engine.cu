@@ -565,21 +565,25 @@ static int launch_thread(hs_engine *E, hs_kernel_run R, const hs_kernel_out &O, 
                                            HS_K4(hs_thread_kernel, HS_WF_LINKED | HS_WF_FAULTS | HS_WF_PROFILE),
                                            HS_K4(hs_thread_kernel, HS_WF_LINKED | HS_WF_FAULTS | HS_WF_HEAPTOP | HS_WF_PROFILE)};
     static const kernel fault_wide_kernels[] = {HS_K4(hs_thread_kernel_wide, HS_WF_FAULTS | HS_WF_PROFILE)};
-    /* time buckets (never with the recorder, never linked), the profile path always compiled in:
-     * [HASH | HEAPTOP ? 2 : 0 | FAULTS ? 4 : 0] and, wide, [HASH | FAULTS ? 2 : 0] */
+    /* time buckets (never with the recorder), the profile path always compiled in:
+     * [HASH | HEAPTOP ? 2 : 0 | FAULTS ? 4 : 0 | LINKED ? 8 : 0] and, wide (never linked), [HASH | FAULTS ? 2 : 0] */
 #define HS_TB_(F) hs_thread_bucket_kernel<HS_WF_BUCKETS | HS_WF_PROFILE | (F)>
-    static const bucket_kernel bucket_kernels[] = {HS_TB_(0), HS_TB_(HS_WF_HASH), HS_TB_(HS_WF_HEAPTOP), HS_TB_(HS_WF_HEAPTOP | HS_WF_HASH),
-                                            HS_TB_(HS_WF_FAULTS), HS_TB_(HS_WF_FAULTS | HS_WF_HASH),
-                                            HS_TB_(HS_WF_FAULTS | HS_WF_HEAPTOP), HS_TB_(HS_WF_FAULTS | HS_WF_HEAPTOP | HS_WF_HASH)};
+#define HS_TB8_(L) HS_TB_(L), HS_TB_((L) | HS_WF_HASH), HS_TB_((L) | HS_WF_HEAPTOP), HS_TB_((L) | HS_WF_HEAPTOP | HS_WF_HASH),         \
+                   HS_TB_((L) | HS_WF_FAULTS), HS_TB_((L) | HS_WF_FAULTS | HS_WF_HASH),                                               \
+                   HS_TB_((L) | HS_WF_FAULTS | HS_WF_HEAPTOP), HS_TB_((L) | HS_WF_FAULTS | HS_WF_HEAPTOP | HS_WF_HASH)
+    static const bucket_kernel bucket_kernels[] = {HS_TB8_(0), HS_TB8_(HS_WF_LINKED)};
+#undef HS_TB8_
 #undef HS_TB_
 #define HS_TBW_(F) hs_thread_bucket_kernel_wide<HS_WF_BUCKETS | HS_WF_PROFILE | (F)>
     static const bucket_kernel bucket_wide_kernels[] = {HS_TBW_(0), HS_TBW_(HS_WF_HASH), HS_TBW_(HS_WF_FAULTS), HS_TBW_(HS_WF_FAULTS | HS_WF_HASH)};
 #undef HS_TBW_
     /* with percentiles, the same order */
 #define HS_TP_(F) hs_thread_bucket_kernel<HS_WF_BUCKETS | HS_WF_BUCKET_PCT | HS_WF_PROFILE | (F)>
-    static const pct_kernel pct_kernels[] = {HS_TP_(0), HS_TP_(HS_WF_HASH), HS_TP_(HS_WF_HEAPTOP), HS_TP_(HS_WF_HEAPTOP | HS_WF_HASH),
-                                             HS_TP_(HS_WF_FAULTS), HS_TP_(HS_WF_FAULTS | HS_WF_HASH),
-                                             HS_TP_(HS_WF_FAULTS | HS_WF_HEAPTOP), HS_TP_(HS_WF_FAULTS | HS_WF_HEAPTOP | HS_WF_HASH)};
+#define HS_TP8_(L) HS_TP_(L), HS_TP_((L) | HS_WF_HASH), HS_TP_((L) | HS_WF_HEAPTOP), HS_TP_((L) | HS_WF_HEAPTOP | HS_WF_HASH),         \
+                   HS_TP_((L) | HS_WF_FAULTS), HS_TP_((L) | HS_WF_FAULTS | HS_WF_HASH),                                               \
+                   HS_TP_((L) | HS_WF_FAULTS | HS_WF_HEAPTOP), HS_TP_((L) | HS_WF_FAULTS | HS_WF_HEAPTOP | HS_WF_HASH)
+    static const pct_kernel pct_kernels[] = {HS_TP8_(0), HS_TP8_(HS_WF_LINKED)};
+#undef HS_TP8_
 #undef HS_TP_
 #define HS_TPW_(F) hs_thread_bucket_kernel_wide<HS_WF_BUCKETS | HS_WF_BUCKET_PCT | HS_WF_PROFILE | (F)>
     static const pct_kernel pct_wide_kernels[] = {HS_TPW_(0), HS_TPW_(HS_WF_HASH), HS_TPW_(HS_WF_FAULTS), HS_TPW_(HS_WF_FAULTS | HS_WF_HASH)};
@@ -591,7 +595,7 @@ static int launch_thread(hs_engine *E, hs_kernel_run R, const hs_kernel_out &O, 
     if (!wide) fl |= (R.heap_top ? HS_WF_HEAPTOP : 0) | (linked ? HS_WF_LINKED : 0);
     const hs_launch_info info = {3, wide ? (uint32_t)HS_KERNEL_THREAD_WIDE : (uint32_t)HS_KERNEL_THREAD, (uint32_t)fl,
                                  R.lane_stride, R.heap_top, tblocks, HS_THREAD_BLOCK, (uint32_t)dyn_smem};
-    const uint32_t bi = (fl & HS_WF_HASH) | ((fl & HS_WF_HEAPTOP) ? 2 : 0) | ((fl & HS_WF_FAULTS) ? 4 : 0);
+    const uint32_t bi = (fl & HS_WF_HASH) | ((fl & HS_WF_HEAPTOP) ? 2 : 0) | ((fl & HS_WF_FAULTS) ? 4 : 0) | ((fl & HS_WF_LINKED) ? 8 : 0);
     const uint32_t wbi = (fl & HS_WF_HASH) | ((fl & HS_WF_FAULTS) ? 2 : 0);
     if (fl & HS_WF_BUCKET_PCT)
         return timed_launch(E, info, wide ? pct_wide_kernels[wbi] : pct_kernels[bi], M, R, (unsigned char *)E->d_state.p,
@@ -876,7 +880,10 @@ int hs_run(hs_engine *E, const hs_run_params *p)
     const size_t bkt_records = E->bkt_n ? (size_t)n * E->bkt_rows * ((size_t)E->bkt_n + 1) : 0;
     const size_t bkt_vals = bkt_records && E->bkt_cap ? (size_t)n * E->bkt_rows * E->bkt_cap : 0;     /* percentile value buffers */
     if (E->bkt_n) {
-        if (linked) return fail(HS_ERR_INVALID, "time buckets are not available on the windows of a linked partition");
+        /* a linked window resumes the partition's accumulators from their records like any window (hs_bucket_begin), so
+         * only the upload path is checked: the partitions of a linked run come through hs_partition_upload */
+        if (linked && !E->partition)
+            return fail(HS_ERR_INVALID, "time buckets on the windows of a linked partition need a model uploaded with hs_partition_upload");
         if (p->record_cap || p->sample_cap || p->service_cap)
             return fail(HS_ERR_INVALID, "time buckets are a summary-mode output: run them without recorder rings (record_cap, sample_cap, service_cap = 0)");
         /* every sample up to end_ns must fall before bucket n: then only the one event processed past end_ns can reach it */

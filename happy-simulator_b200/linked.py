@@ -118,9 +118,15 @@ class LinkedRun:
         if self.coordinator is not None:
             self.coordinator.close()
 
-    def run(self, *, seed, end_ns, n_replicas=1, replica_index_base=0, caps=None, flags=A.HS_RUN_ORDER_HASH, queue_ring=0):
+    def run(self, *, seed, end_ns, n_replicas=1, replica_index_base=0, caps=None, flags=A.HS_RUN_ORDER_HASH, queue_ring=0,
+            buckets=None, bucket_sample_cap=0):
         """caps: per-partition dicts of record_cap / sample_cap / service_cap (or one dict for all).  Returns the
-        per-partition outputs (Engine.read_outputs) and (delivered, lost, overflowed) per replica."""
+        per-partition outputs (Engine.read_outputs) and (delivered, lost, overflowed) per replica.
+
+        ``buckets=(width_s, n)`` (checked by the caller, with no recorder rings in ``caps``) buckets the samples of
+        every partition that has a Sink, tracker or Probe row; ``bucket_sample_cap`` > 0 adds their p50 / p99.  Those
+        partitions' outputs get the keys of ``buckets.read_outputs``; the other partitions run as without buckets."""
+        from . import buckets as _buckets
         from . import engine as _engine
         lm, nP = self.lm, self.lm.n_partitions
         if self.coordinator is not None:
@@ -130,16 +136,28 @@ class LinkedRun:
         caps = caps or {}
         link_args = [lm.link_descs(q) for q in range(nP)]
         ends = lm.window_ends(end_ns)
-        for w, wend in enumerate(ends):
-            for q, e in enumerate(self.engines):
-                c = caps[q] if isinstance(caps, (list, tuple)) else caps
-                e.run(_engine.make_params(seed=seed, end_ns=wend, n_replicas=n_replicas, rid_base=q, rid_stride=nP + 1,
-                                          replica_index_base=replica_index_base, engine=3, resume=1 if w else 0,
-                                          flags=flags | A.HS_RUN_LINKED, queue_ring=queue_ring, **c))
-            for q, e in enumerate(self.engines):
-                arr, dst = link_args[q]
-                if dst:
-                    self.coordinator.exchange(e, arr, [self.engines[d] for d in dst])
-        self.windows = len(ends)
-        outs = [e.read_outputs() for e in self.engines]
+        bucketed = [q for q, m in enumerate(lm.models) if buckets is not None and _buckets.rows(m)]
+        try:
+            for q in bucketed:
+                self.engines[q].set_buckets(*buckets)
+                self.engines[q].set_bucket_percentiles(bucket_sample_cap)
+            for w, wend in enumerate(ends):
+                for q, e in enumerate(self.engines):
+                    c = caps[q] if isinstance(caps, (list, tuple)) else caps
+                    e.run(_engine.make_params(seed=seed, end_ns=wend, n_replicas=n_replicas, rid_base=q, rid_stride=nP + 1,
+                                              replica_index_base=replica_index_base, engine=3, resume=1 if w else 0,
+                                              flags=flags | A.HS_RUN_LINKED, queue_ring=queue_ring, **c))
+                for q, e in enumerate(self.engines):
+                    arr, dst = link_args[q]
+                    if dst:
+                        self.coordinator.exchange(e, arr, [self.engines[d] for d in dst])
+            self.windows = len(ends)
+            outs = [e.read_outputs() for e in self.engines]
+            for q in bucketed:
+                objs = lm.objects[q] if lm.objects else [None] * lm.models[q].n_entities
+                outs[q].update(_buckets.read_outputs(self.engines[q], buckets, bucket_sample_cap, lm.models[q], objs))
+        finally:
+            for e in self.engines:          # the engines may run again without buckets
+                e.set_bucket_percentiles(0)
+                e.set_buckets(0.0, 0)
         return outs, self.coordinator.read()

@@ -252,9 +252,10 @@ class ParallelSimulation:
     link_buffer = 256        # cross-partition events one replica may emit per window (class default; overflow is reported)
     queue_ring = 0           # device slots per server queue of a linked run (0: the engine's default); grown and re-run on overflow
 
-    def _run_linked(self, n_replicas: int = 1, replica_index_base: int = 0):
+    def _run_linked(self, n_replicas: int = 1, replica_index_base: int = 0, buckets=None, bucket_sample_cap: int = 0):
         from . import _abi as A
-        from .api import Instant
+        from . import buckets as _buckets
+        from .api import EnsembleStatusError, Instant
         from .linked import LinkedRun
         from .lowering import refresh_fault_cancellation
         lm = self._linked
@@ -262,9 +263,13 @@ class ParallelSimulation:
             refresh_fault_cancellation(m)
         t0 = _time.monotonic()
         run = LinkedRun(lm, device=self._device)
+        cap = bucket_sample_cap
         try:
             caps = []
             for m, rate in zip(lm.models, _reaching_rates(lm)):
+                if buckets is not None:     # the buckets are the run's time series: no recorder rings
+                    caps.append(dict(sample_cap=0, service_cap=0, record_cap=0))
+                    continue
                 ev = max(64, int(_events_bound(rate, m.inbox_cap, self._end_ns)))
                 many = len(m.ids_of(A.HS_ENT_SINK)) + len(m.ids_of(A.HS_ENT_PROBE)) > 1 or len(m.ids_of(A.HS_ENT_SERVER)) > 1
                 caps.append(dict(sample_cap=ev, service_cap=ev, record_cap=8 * ev if many else 0))   # records tell the sinks / servers apart
@@ -274,23 +279,33 @@ class ParallelSimulation:
             # too small and run the whole thing again (every window starts from scratch: resume = 0 at window 0, a fresh
             # coordinator) instead of handing that to the caller.  Growth happens before an attempt, so `ring` and
             # `caps` are always what the last attempt ran with.
+            # With percentiles, a time bucket that outgrew the sample capacity is no failure either: the whole run is
+            # repeated once with the capacity that holds every bucket (as Simulation.run_ensemble's "grow").
             ring = int(getattr(self, "queue_ring", 0) or 0)
-            queue_full, short = False, []
+            ok = _TIES | (A.HS_ST_BUCKET_OVERFLOW if cap else 0)
+            queue_full, short, cap_short, cap_grown = False, [], False, False
             for attempt in range(6):
                 if queue_full:
                     ring = max(512, 4 * ring)
-                for q, cap, n in short:
-                    caps[q][cap] = 2 * n + 64
+                for q, c, n in short:
+                    caps[q][c] = 2 * n + 64
+                if cap_short:
+                    cap = max(_buckets.sample_cap_needed(o["buckets"]) for o in outs if "buckets" in o)
+                    cap_grown = True
+                bk = dict(buckets=buckets, bucket_sample_cap=cap) if buckets is not None else {}
                 outs, (delivered, lost, over) = run.run(seed=self._seed, end_ns=self._end_ns, n_replicas=n_replicas,
-                                                        replica_index_base=replica_index_base, caps=caps, flags=0, queue_ring=ring)
+                                                        replica_index_base=replica_index_base, caps=caps, flags=0, queue_ring=ring,
+                                                        **bk)
                 status = 0
                 for o in outs:
                     status |= int(np.bitwise_or.reduce(o["summaries"]["status"])) if len(o["summaries"]) else 0
-                clean = not (status & ~_TIES) and not over.any()
-                queue_full = bool(status & A.HS_ST_QUEUE_OVERFLOW and not (status & ~(A.HS_ST_QUEUE_OVERFLOW | _TIES))
+                clean = not (status & ~ok) and not over.any()
+                queue_full = bool(status & A.HS_ST_QUEUE_OVERFLOW and not (status & ~(A.HS_ST_QUEUE_OVERFLOW | ok))
                                   and not over.any())
-                short = _short_rings(outs, caps) if clean else []     # counts of a run that stopped early mean nothing
-                if not (queue_full or short):
+                # counts of a run that stopped early mean nothing; a bucketed run has no rings
+                short = _short_rings(outs, caps) if clean and buckets is None else []
+                cap_short = clean and bool(status & A.HS_ST_BUCKET_OVERFLOW) and not cap_grown
+                if not (queue_full or short or cap_short):
                     break
             self.last_queue_ring = ring
         finally:
@@ -302,7 +317,7 @@ class ParallelSimulation:
                                f"{caps[q][cap]} device slots ({cap}) in the last of {attempt + 1} attempts; the ring "
                                "wrapped, so its results are not published")
         wall = _time.monotonic() - t0
-        bad = [(lm.names[q], int(s)) for q, o in enumerate(outs) for s in o["summaries"]["status"] if int(s) & ~_TIES]
+        bad = [(lm.names[q], int(s)) for q, o in enumerate(outs) for s in o["summaries"]["status"] if int(s) & ~ok]
         if bad or over.any():
             bits = 0
             for _, s_ in bad:
@@ -316,6 +331,12 @@ class ParallelSimulation:
                 why.append(f"status bits {bits & ~(A.HS_ST_QUEUE_OVERFLOW | A.HS_ST_LINK_OVERFLOW | _TIES):#x}")
             raise RuntimeError(f"linked run did not complete cleanly: partition status {bad[:4]}, inbox overflows {int(over.sum())}: "
                                + "; ".join(why))
+        if status & A.HS_ST_BUCKET_OVERFLOW:
+            st = np.stack([o["summaries"]["status"] for o in outs])
+            need = max(_buckets.sample_cap_needed(o["buckets"]) for o in outs if "buckets" in o)
+            n_over = int((np.bitwise_or.reduce(st, axis=0) & A.HS_ST_BUCKET_OVERFLOW != 0).sum())
+            raise EnsembleStatusError(f"{n_over} of {n_replicas} replicas had a time bucket with more samples than "
+                                      f"bucket_sample_cap={cap}; pass bucket_sample_cap={need}", st)
         self.link_ties = int(sum(int(s) & A.HS_ST_LINK_TIE != 0 for o in outs for s in o["summaries"]["status"]))
         self.fault_ties = int(sum(int(s) & A.HS_ST_FAULT_TIE != 0 for o in outs for s in o["summaries"]["status"]))
         self.last_outputs, self.last_delivered, self.last_lost = outs, delivered, lost
@@ -342,13 +363,23 @@ class ParallelSimulation:
             partition_wall_times={nm: wall / n for nm in summaries}, speedup=1.0, parallelism_efficiency=1.0 / n if n else 1.0,
             total_windows=windows, total_cross_partition_events=int(delivered[0]), window_size_s=lm.window_s)
 
-    def run_ensemble(self, n_replicas: int, replica_index_base: int = 0):
+    def run_ensemble(self, n_replicas: int, replica_index_base: int = 0, *, buckets=None, bucket_percentiles: bool = False,
+                     bucket_sample_cap: int = 64):
         """Linked partitions only: n replicas of the whole ParallelSimulation in one set of launches.  Returns
         {partition name: per-replica outputs (Engine.read_outputs)}, delivered and lost cross-partition events per
-        replica."""
+        replica.
+
+        ``buckets=(width_s, n)``, ``bucket_percentiles`` and ``bucket_sample_cap`` are those of
+        ``Simulation.run_ensemble``: every partition with a Sink, tracker or Probe gets its time buckets (and p50 / p99)
+        under the same keys (one cell), and ``buckets.bucketed_data(outs[name], obj, replica)`` reads them.  Such a run
+        keeps no recorder rings, so its memory does not grow with the horizon.  A bucket with more than
+        ``bucket_sample_cap`` samples makes the run repeat once with the capacity that holds them all."""
+        from . import buckets as _buckets
         if self._linked is None:
             raise UnsupportedModelError("run_ensemble is for partitions joined by PartitionLinks")
-        outs, delivered, lost, wall, windows = self._run_linked(n_replicas, replica_index_base)     # a rank's shard: base = rank * n
+        spec = _buckets.check_spec(buckets, self._end_ns) if buckets is not None else None
+        cap = _buckets.check_sample_cap(bucket_sample_cap, spec) if bucket_percentiles else 0
+        outs, delivered, lost, wall, windows = self._run_linked(n_replicas, replica_index_base, spec, cap)   # a rank's shard: base = rank * n
         return {n: o for n, o in zip(self._linked.names, outs)}, delivered, lost
 
     def _run_independent(self) -> ParallelSimulationSummary:

@@ -520,8 +520,10 @@ int hs_read_inbox(hs_engine *e, hs_xevent *buf, uint32_t *counts);
  * separately).  hs_run refuses a bucketed run whose end time falls into bucket n or later (n * width_s must exceed
  * the end time), a run with recorder rings (record_cap, sample_cap or service_cap: buckets are the summary-mode
  * series; the rings stay the record-mode path), a window of a linked partition (HS_RUN_LINKED or a model with
- * REMOTE rows), and a resume whose bucket configuration differs from the paused run's.  It checks the size of the
- * records against the free device memory before it allocates them. */
+ * REMOTE rows) whose model did not come through hs_partition_upload, and a resume whose bucket configuration differs
+ * from the paused run's.  The windows of a linked run keep their buckets like those of a windowed run: every window
+ * passes the same configuration, and the last one's records are the whole run's.  It checks the size of the records
+ * against the free device memory before it allocates them. */
 int hs_set_buckets(hs_engine *e, double width_s, uint32_t n);
 
 /* Copy the last run's buckets: out[n_replicas][rows][n + 1] (see hs_set_buckets) and past_end[n_replicas][rows], the
