@@ -512,7 +512,10 @@ static void handle(orun *R, oev *e)
     }
 }
 
-typedef struct { const double *targets; uint64_t n_targets; const double *service; uint64_t n_service; } otrace;
+/* one replica's rows of externally supplied draws (NULL: that stream comes from Philox), and where to report how many
+ * draws of each stream the replica asked for (the cursors' final values; NULL: not reported) */
+typedef struct { const double *targets; uint64_t n_targets; const double *service; uint64_t n_service;
+                 uint64_t *arr_used, *svc_used; } otrace;
 
 /* Simulation.__init__ of one replica: entity state, output cursors, the sources' first ticks */
 static void orun_init(orun *Rp, const hs_model_desc *m, const hs_run_params *p, uint32_t r,
@@ -665,6 +668,8 @@ static void run_replica(const hs_model_desc *m, const hs_run_params *p, uint32_t
      * than the window end; resume is not modelled here -- a paused prefix is compared against the device's. */
     const int windowed = (p->window_end_ns >= 0 && p->window_end_ns < p->end_ns);
     orun_until(&R, p->end_ns, windowed ? p->window_end_ns : -1);
+    if (tr && tr->arr_used) *tr->arr_used = R.np_cursor;
+    if (tr && tr->svc_used) *tr->svc_used = R.py_cursor;
     orun_finish(&R);
 }
 
@@ -803,16 +808,37 @@ int hs_oracle_bench(const hs_model_desc *m, const hs_run_params *p, int n_thread
     return HS_OK;
 }
 
-/* One replica driven by externally supplied draws: arrival target areas
- * (-log(1-U), poisson_arrival.py:31) and service samples (random.expovariate,
- * exponential.py:43) captured from the reference's stock generators. */
+/* Replicas driven by externally supplied draws: arrival target areas (-log(1-U), poisson_arrival.py:31) and
+ * service samples (random.expovariate, exponential.py:43) captured from the reference's stock generators.  The
+ * draws are laid out as hs_set_trace lays them out, one row per replica slot: targets[n_replicas][n_targets],
+ * service[n_replicas][n_service]; a stream with no draws (NULL or n = 0) comes from Philox, as on the device.  The
+ * cell of a replica follows replica_index_base and replicas_per_cell, as in hs_oracle_run.  A replica that asks for
+ * a draw past the end of its row gets a target of 1e300 (no further arrival, an unbounded service time) and runs on;
+ * arr_used / svc_used (per replica slot, each optional) receive how many draws of each stream the replica asked
+ * for, so a caller learns what every replica needed.  Replicas [r0, r1) only, so Python can spread a batch over
+ * threads (r1 is clamped to n_replicas). */
+int hs_oracle_run_trace_range(const hs_model_desc *m, const hs_run_params *p, const hs_outputs *out,
+                              const double *targets, uint64_t n_targets, const double *service, uint64_t n_service,
+                              uint32_t r0, uint32_t r1, uint64_t *arr_used, uint64_t *svc_used)
+{
+    if (!m || !p || !out || m->abi_version != HS_ABI_VERSION) return HS_ERR_INVALID;
+    if (!targets) n_targets = 0;
+    if (!service) n_service = 0;
+    for (uint32_t r = r0; r < r1 && r < p->n_replicas; ++r) {
+        otrace tr = { n_targets ? targets + (size_t)r * n_targets : NULL, n_targets,
+                      n_service ? service + (size_t)r * n_service : NULL, n_service,
+                      arr_used ? arr_used + r : NULL, svc_used ? svc_used + r : NULL };
+        run_replica(m, p, r, out, &tr);
+    }
+    return HS_OK;
+}
+
+/* Every replica of hs_oracle_run_trace_range, without the draw counts. */
 int hs_oracle_run_trace(const hs_model_desc *m, const hs_run_params *p, const hs_outputs *out,
                         const double *targets, uint64_t n_targets, const double *service, uint64_t n_service)
 {
-    if (!m || !p || !out || m->abi_version != HS_ABI_VERSION || p->n_replicas != 1) return HS_ERR_INVALID;
-    otrace tr = { targets, n_targets, service, n_service };
-    run_replica(m, p, 0, out, &tr);
-    return HS_OK;
+    if (!p) return HS_ERR_INVALID;
+    return hs_oracle_run_trace_range(m, p, out, targets, n_targets, service, n_service, 0, p->n_replicas, NULL, NULL);
 }
 
 int hs_sketch_layout(const hs_model_desc *m, uint64_t *per_replica, uint64_t *merged, uint64_t *total, uint64_t *merged_total)

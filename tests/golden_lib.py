@@ -114,3 +114,24 @@ def check_linked_partition(z, q, got, r=0):
         assert got["service_samples"][r][:n].tobytes() == z[pre + "service_samples"].tobytes(), f"partition {q}: service samples differ"
     if pre + "sketch_state" in z.files and len(z[pre + "sketch_state"]):
         assert got["sketches"][r].tobytes() == z[pre + "sketch_state"].tobytes(), f"partition {q}: sketch state differs"
+
+
+def stock_ensemble_caps(z):
+    """Ring capacities that retain the whole run of every replica of a stock-ensemble fixture."""
+    return dict(record_cap=int(z["n_records"].max()) + 1, sample_cap=int(z["n_samples"].max()) + 1,
+                service_cap=int(z["n_service"].max()) + 1)
+
+
+def check_stock_ensemble(z, k, got, r):
+    """Replica k of a stock-ensemble fixture (tests/golden/gen_stock_ensemble_golden.py) against replica r of an oracle /
+    engine result whose rings retain the whole run (stock_ensemble_caps)."""
+    s, ws = got["summaries"][r], z["summaries"][k]
+    for f in ("events_processed", "final_time_ns", "order_hash", "heap_left", "n_sink_samples", "n_service_samples"):
+        assert int(s[f]) == int(ws[f]), (k, f, int(s[f]), int(ws[f]))
+    assert got["entity_stats"][r].tobytes() == z["entity_stats"][k].tobytes(), f"seed {k}: entity statistics differ"
+    n = min(int(z["n_records"][k]), z["records"].shape[1])
+    assert got["records"][r][:n].tobytes() == z["records"][k][:n].tobytes(), f"seed {k}: event records differ"
+    n = int(z["n_samples"][k])
+    assert got["sink_samples"][r][:n].tobytes() == z["sink_samples"][k][:n].tobytes(), f"seed {k}: sink samples differ"
+    n = int(z["n_service"][k])
+    assert got["service_samples"][r][:n].tobytes() == z["service_samples"][k][:n].tobytes(), f"seed {k}: service times differ"

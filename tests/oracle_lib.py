@@ -30,6 +30,9 @@ def lib():
         L.hs_oracle_run_trace.argtypes = [C.POINTER(A.ModelDesc), C.POINTER(A.RunParams), C.POINTER(A.Outputs),
                                           C.POINTER(C.c_double), C.c_uint64, C.POINTER(C.c_double), C.c_uint64]
         L.hs_oracle_run_trace.restype = C.c_int
+        L.hs_oracle_run_trace_range.argtypes = list(L.hs_oracle_run_trace.argtypes) + [
+            C.c_uint32, C.c_uint32, C.POINTER(C.c_uint64), C.POINTER(C.c_uint64)]
+        L.hs_oracle_run_trace_range.restype = C.c_int
         L.hs_cpu_uniform.argtypes = [C.c_uint64, C.c_uint32, C.c_uint32, C.c_uint64]
         L.hs_cpu_uniform.restype = C.c_double
         for n in ("hs_cpu_log", "hs_cpu_exp1"):
@@ -208,14 +211,32 @@ class OracleLinkedRun:
         return outs, (delivered, lost, np.zeros(n_replicas, np.uint64))
 
 
-def oracle_run_trace(model, p: A.RunParams, targets, service):
-    """One replica fed with externally captured draws (the reference's stock RNG outputs)."""
+def _trace_rows(x, n):
+    """Draws of one stream as [n_replicas, n_draws] float64 rows (a 1-D array: the row of a single replica)."""
+    a = np.ascontiguousarray(np.zeros((n, 0)) if x is None else x, dtype=np.float64)
+    a = a[None, :] if a.ndim == 1 else a
+    assert a.ndim == 2 and a.shape[0] == n, (a.shape, n)
+    return a
+
+
+def oracle_run_trace(model, p: A.RunParams, targets, service, chunk: int = 64):
+    """Replicas fed with externally captured draws (the reference's stock RNG outputs): ``targets`` and ``service``
+    hold one row per replica slot, [n_replicas, n] as ``Engine.set_trace`` takes them (a 1-D array is the row of a
+    single replica; None or zero columns leave that stream to Philox).  Returns the output buffers plus
+    ``arr_used`` / ``svc_used``: how many draws of each stream every replica asked for, whether or not its row had
+    them (a draw past the end of a row is a target of 1e300).  Runs on a thread pool in slices of ``chunk``."""
     d = model.desc()
-    bufs, o = alloc_outputs(model.n_entities, p)
-    t = np.ascontiguousarray(targets, dtype=np.float64)
-    s = np.ascontiguousarray(service, dtype=np.float64)
-    rc = lib().hs_oracle_run_trace(C.byref(d), C.byref(p), C.byref(o),
-                                   t.ctypes.data_as(C.POINTER(C.c_double)), len(t),
-                                   s.ctypes.data_as(C.POINTER(C.c_double)), len(s))
-    assert rc == 0, rc
+    n = p.n_replicas
+    bufs, o = alloc_outputs(model.n_entities, p, model.sketch_layout()[2])
+    t, s = _trace_rows(targets, n), _trace_rows(service, n)
+    bufs["arr_used"], bufs["svc_used"] = np.zeros(n, np.uint64), np.zeros(n, np.uint64)
+    dp = C.POINTER(C.c_double)
+    up = C.POINTER(C.c_uint64)
+
+    def part(r0):
+        assert lib().hs_oracle_run_trace_range(C.byref(d), C.byref(p), C.byref(o), t.ctypes.data_as(dp), t.shape[1],
+                                               s.ctypes.data_as(dp), s.shape[1], r0, min(n, r0 + chunk),
+                                               bufs["arr_used"].ctypes.data_as(up), bufs["svc_used"].ctypes.data_as(up)) == 0
+
+    _pool_map(part, range(0, n, chunk))
     return bufs
