@@ -65,10 +65,32 @@ typedef struct oev {
     double svc_s;        /* CONTINUATION: the service time the generator yielded  */
     int32_t stage;       /* CONTINUATION at a CachingServer: which yield resumes (1, 2, 3) | was_in_cache << 8 */
     uint64_t payload_idx;/* DELIVER: _sort_index of the payload Event it carries  */
+#ifdef HS_ORACLE_HIGH_WATER
+    int32_t hw_future;   /* scheduled strictly later than its creation, or at the bootstrap / a barrier */
+#endif
 } oev;
 
 /* ---- CPython heapq (Lib/heapq.py: heappush/_siftdown, heappop/_siftup) -- */
+#ifdef HS_ORACLE_HIGH_WATER
+/* High-water marks of the structures the device bounds, kept only in the instrumented build (-DHS_ORACLE_HIGH_WATER,
+ * tests/high_water_lib.py).  The reference's heap has no limit; on the device an event created at or before the
+ * clock joins the same-timestamp ("now") tier (HS_W_PUSH: t <= now) and every other event takes a future-event slot,
+ * as do the bootstrap events and what a barrier delivers.  One row of HS_HW_FIELDS + n_entities counters per replica:
+ *   HS_HW_NOW       most now-tier events pending at once (the event being handled is not pending)
+ *   HS_HW_NOW_POP   most now-tier events pending when a future event is popped (the warp engine moves that event
+ *                   into its now tier before handling it, so it needs a free entry then)
+ *   HS_HW_FUTURE    most future events pending at once
+ *   HS_HW_OUTBOX    linked runs: most cross-partition sends in one window, the ones the full outbox dropped included
+ *   HS_HW_INBOX     linked runs: most events delivered into this partition at one barrier
+ *   HS_HW_FIELDS+i  entity i: the longest its queue was right after an enqueue (a bounded queue drops first) */
+enum { HS_HW_NOW, HS_HW_NOW_POP, HS_HW_FUTURE, HS_HW_OUTBOX, HS_HW_INBOX, HS_HW_FIELDS };
+typedef struct { oev *a; size_t n, cap;
+                 int64_t clock;            /* time of the event being handled; INT64_MIN at the bootstrap and a barrier */
+                 uint32_t n_now, n_future, hw[HS_HW_FIELDS]; } oheap;
+#define HS_HW_MAX(x, v) do { if ((v) > (x)) (x) = (v); } while (0)
+#else
 typedef struct { oev *a; size_t n, cap; } oheap;
+#endif
 
 static int ev_lt(const oev *x, const oev *y)    /* Event.__lt__, event.py:337-344 */
 {
@@ -110,6 +132,10 @@ static void heap_push(oheap *h, const oev *e)
         h->a = (oev *)realloc(h->a, h->cap * sizeof(oev));
     }
     h->a[h->n++] = *e;
+#ifdef HS_ORACLE_HIGH_WATER
+    if ((h->a[h->n - 1].hw_future = e->time > h->clock)) { h->n_future++; HS_HW_MAX(h->hw[HS_HW_FUTURE], h->n_future); }
+    else { h->n_now++; HS_HW_MAX(h->hw[HS_HW_NOW], h->n_now); }
+#endif
     heap_siftdown(h, 0, h->n - 1);
 }
 
@@ -152,6 +178,9 @@ typedef struct oent {
     int64_t cache_hits, cache_misses, cache_size;
     int cache_own;                    /* cache_ins is a private allocation (no hs_outputs.sketches buffer)   */
     uint8_t *sk_state;                /* this replica's registers / counters (in hs_outputs.sketches) */
+#ifdef HS_ORACLE_HIGH_WATER
+    uint32_t hw_queue;                /* longest queue right after an enqueue                                */
+#endif
 } oent;
 
 typedef struct orun {
@@ -178,6 +207,9 @@ typedef struct orun {
     hs_xevent *outbox; uint32_t outbox_n, outbox_cap;
     uint32_t r;                           /* replica slot in the outputs                                */
     const hs_outputs *out;
+#ifdef HS_ORACLE_HIGH_WATER
+    uint32_t hw_sent, hw_received;        /* cross-partition sends / deliveries in the current window   */
+#endif
 } orun;
 
 static void q_push(oent *s, const oreq *r)
@@ -326,6 +358,9 @@ static void handle(orun *R, oev *e)
         } else {
             oreq r; r.created_at = e->created_at; r.idx = e->idx; r.req_id = e->req_id; r.key = e->key;
             q_push(E, &r);
+#ifdef HS_ORACLE_HIGH_WATER
+            HS_HW_MAX(E->hw_queue, (uint32_t)E->q_len);
+#endif
             E->accepted++;
             if (was_empty) {
                 oev n = new_event(R, R->now, HS_EV_NOTIFY, e->ent);
@@ -437,6 +472,9 @@ static void handle(orun *R, oev *e)
                 /* the partition's event router (routing.py:40-61): a target outside this partition -> the event,
                  * already constructed (its sort index is spent), goes to the outbox with the current time */
                 R->ents[E->d.target].received++;
+#ifdef HS_ORACLE_HIGH_WATER
+                R->hw_sent++; HS_HW_MAX(R->heap.hw[HS_HW_OUTBOX], R->hw_sent);
+#endif
                 if (R->outbox_n < R->outbox_cap) {
                     hs_xevent *x = &R->outbox[R->outbox_n++];
                     x->time_ns = R->now; x->sort_index = f.idx; x->created_ns = f.created_at; x->aux = 0;
@@ -523,6 +561,9 @@ static void orun_init(orun *Rp, const hs_model_desc *m, const hs_run_params *p, 
 {
 #define R (*Rp)
     memset(&R, 0, sizeof R);
+#ifdef HS_ORACLE_HIGH_WATER
+    R.heap.clock = INT64_MIN;
+#endif
     R.m = m; R.p = p; R.r = r; R.out = out;
     if (tr) { R.trace_targets = tr->targets; R.n_trace_targets = tr->n_targets;
               R.trace_service = tr->service; R.n_trace_service = tr->n_service; }
@@ -603,8 +644,15 @@ static void orun_until(orun *Rp, int64_t end_ns, int64_t cut_ns)
         if (p->max_events > 0 && R.processed >= p->max_events) { R.status |= HS_ST_EVENT_LIMIT; break; }
         if (cut_ns >= 0 && R.heap.a[0].time > cut_ns) break;
         oev e = heap_pop(&R.heap);
+#ifdef HS_ORACLE_HIGH_WATER
+        if (e.hw_future) { R.heap.n_future--; HS_HW_MAX(R.heap.hw[HS_HW_NOW_POP], R.heap.n_now); }
+        else R.heap.n_now--;
+#endif
         if (e.time < R.now) continue;     /* "time travel": skipped, not counted (simulation.py:479-489) */
         R.now = e.time;
+#ifdef HS_ORACLE_HIGH_WATER
+        R.heap.clock = R.now;
+#endif
         uint64_t w1 = hs_record_word1(e.idx, (uint32_t)e.kind, (uint32_t)e.ent);
         R.hash = hs_hash_step(R.hash, e.time, w1);
         if (R.rec && p->record_cap) {
@@ -616,6 +664,9 @@ static void orun_until(orun *Rp, int64_t end_ns, int64_t cut_ns)
         R.processed++;
         handle(&R, &e);
     }
+#ifdef HS_ORACLE_HIGH_WATER
+    R.heap.clock = INT64_MIN;             /* what a barrier delivers next is scheduled from outside the run */
+#endif
 #undef R
 }
 
@@ -659,6 +710,19 @@ static void orun_finish(orun *Rp)
 #undef R
 }
 
+#ifdef HS_ORACLE_HIGH_WATER
+/* where run_replica / hs_oracle_run_linked write the rows (set by the *_high_water entry points; one per thread, so
+ * slices of an ensemble can run on a thread pool) */
+static _Thread_local uint32_t *hw_rows;
+static _Thread_local uint32_t *const *hw_part_rows;
+
+static void hw_publish(const orun *R, uint32_t *row)
+{
+    memcpy(row, R->heap.hw, sizeof R->heap.hw);
+    for (uint32_t i = 0; i < R->m->n_entities; ++i) row[HS_HW_FIELDS + i] = R->ents[i].hw_queue;
+}
+#endif
+
 static void run_replica(const hs_model_desc *m, const hs_run_params *p, uint32_t r,
                         const hs_outputs *out, const otrace *tr)
 {
@@ -670,6 +734,9 @@ static void run_replica(const hs_model_desc *m, const hs_run_params *p, uint32_t
     orun_until(&R, p->end_ns, windowed ? p->window_end_ns : -1);
     if (tr && tr->arr_used) *tr->arr_used = R.np_cursor;
     if (tr && tr->svc_used) *tr->svc_used = R.py_cursor;
+#ifdef HS_ORACLE_HIGH_WATER
+    if (hw_rows) hw_publish(&R, hw_rows + (size_t)r * (HS_HW_FIELDS + m->n_entities));
+#endif
     orun_finish(&R);
 }
 
@@ -717,6 +784,9 @@ int hs_oracle_run_linked(uint32_t n_parts, const hs_model_desc *const *models, c
         }
         for (uint32_t w = 0; w < n_windows; ++w) {
             for (uint32_t q = 0; q < n_parts; ++q) orun_until(&R[q], window_ends[w], -1);      /* 1. EXECUTE */
+#ifdef HS_ORACLE_HIGH_WATER
+            for (uint32_t q = 0; q < n_parts; ++q) R[q].hw_received = 0;
+#endif
             for (uint32_t q = 0; q < n_parts; ++q) {                                            /* 2. EXCHANGE */
                 for (uint32_t k = 0; k < R[q].outbox_n; ++k) {
                     const hs_xevent *x = &R[q].outbox[k];
@@ -736,10 +806,20 @@ int hs_oracle_run_linked(uint32_t n_parts, const hs_model_desc *const *models, c
                     e.created_at = x->created_ns; e.key = x->key; e.lb_hook = -1; e.poll_hook = -1;
                     heap_push(&D->heap, &e);
                     n_del++;
+#ifdef HS_ORACLE_HIGH_WATER
+                    D->hw_received++; HS_HW_MAX(D->heap.hw[HS_HW_INBOX], D->hw_received);
+#endif
                 }
                 R[q].outbox_n = 0;
+#ifdef HS_ORACLE_HIGH_WATER
+                R[q].hw_sent = 0;
+#endif
             }
         }
+#ifdef HS_ORACLE_HIGH_WATER
+        if (hw_part_rows)
+            for (uint32_t q = 0; q < n_parts; ++q) hw_publish(&R[q], hw_part_rows[q] + (size_t)r * (HS_HW_FIELDS + models[q]->n_entities));
+#endif
         for (uint32_t q = 0; q < n_parts; ++q) { free(R[q].outbox); orun_finish(&R[q]); }
         if (delivered) delivered[r] = n_del;
         if (lost) lost[r] = n_lost;
@@ -756,6 +836,32 @@ int hs_oracle_run_range(const hs_model_desc *m, const hs_run_params *p, const hs
     for (uint32_t r = r0; r < r1 && r < p->n_replicas; ++r) run_replica(m, p, r, out, NULL);
     return HS_OK;
 }
+
+#ifdef HS_ORACLE_HIGH_WATER
+/* hs_oracle_run_range that also fills hw[n_replicas][HS_HW_FIELDS + n_entities] (rows [r0, r1) only) */
+int hs_oracle_high_water_range(const hs_model_desc *m, const hs_run_params *p, const hs_outputs *out,
+                               uint32_t r0, uint32_t r1, uint32_t *hw)
+{
+    hw_rows = hw;
+    const int rc = hs_oracle_run_range(m, p, out, r0, r1);
+    hw_rows = NULL;
+    return rc;
+}
+
+/* hs_oracle_run_linked that also fills hw[q][n_replicas][HS_HW_FIELDS + n_entities of partition q] */
+int hs_oracle_high_water_linked(uint32_t n_parts, const hs_model_desc *const *models, const hs_run_params *const *params,
+                                const hs_outputs *const *outs, const hs_link_desc *const *links, const uint32_t *const *link_dst,
+                                const int64_t *window_ends, uint32_t n_windows, uint32_t n_streams,
+                                uint64_t cseed, uint64_t cseed_stride, uint32_t crid_base, uint32_t crid_stride,
+                                uint64_t *delivered, uint64_t *lost, uint32_t *const *hw)
+{
+    hw_part_rows = hw;
+    const int rc = hs_oracle_run_linked(n_parts, models, params, outs, links, link_dst, window_ends, n_windows, n_streams,
+                                        cseed, cseed_stride, crid_base, crid_stride, delivered, lost);
+    hw_part_rows = NULL;
+    return rc;
+}
+#endif
 
 /* CPU anchor for bench.py: n_threads POSIX threads pull replica indices [0, max_replicas) from a shared
  * counter and run them until budget_s of wall time is spent (a replica in progress is finished), all inside
