@@ -31,9 +31,9 @@
 
 #define HS_BUCKET_SLICE 256u        /* replicas per first-stage slice of the cell reduction */
 
-/* The bucket arguments reach the engine kernels as their last parameter, of type hs_bucket_args in the bucket
- * instantiations and of the empty hs_no_bucket_args in every other one: those keep their parameter block (and with it
- * their code) as it was. */
+/* The bucket arguments reach every engine kernel (lane, warp, both thread forms) as its last parameter, of type
+ * hs_bucket_args in the bucket instantiations and of the empty hs_no_bucket_args in every other one, an unused
+ * parameter that changes none of their code. */
 struct hs_bucket_args {
     double w;                       /* width in seconds */
     uint32_t n, rows;               /* buckets per row, bucketed rows (SINK and PROBE rows) */

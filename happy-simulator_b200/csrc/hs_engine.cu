@@ -13,7 +13,9 @@
 #include <cstdlib>
 #include <cstring>
 #include <algorithm>
+#include <array>
 #include <string>
+#include <utility>
 #include <vector>
 
 #include "../../include/hs_b200.h"
@@ -338,22 +340,40 @@ static uint32_t pow2_at_least(uint32_t v) { uint32_t p = 1; while (p < v) p <<= 
 
 /* ---- one launcher per kernel ----------------------------------------------- */
 
+/* A kernel's instantiations as one table indexed by the flag word: entry F is at(F), the instantiation where the
+ * kernel's predicate (hs_lane_built, hs_warp_built, hs_thread_built, hs_thread_wide_built) holds and nullptr elsewhere. */
+template <class At, int... F>
+static std::array<const void *, sizeof...(F)> kernel_table(At at, std::integer_sequence<int, F...>)
+{
+    return {at(std::integral_constant<int, F>())...};
+}
+template <int N, class At>
+static std::array<const void *, N> kernel_table(At at) { return kernel_table(at, std::make_integer_sequence<int, N>()); }
+
+/* An engine kernel's last argument, of the type the bucket bits of its flag word give it (hs_bucket_args_of): the
+ * percentile arguments, their hs_bucket_args base, or the empty hs_no_bucket_args. */
+static void *bucket_arg(const hs_bucket_pct_args &BK, bool buckets, bool pct)
+{
+    static const hs_no_bucket_args none = {};
+    return pct ? (void *)&BK : buckets ? (void *)static_cast<const hs_bucket_args *>(&BK) : (void *)&none;
+}
+
 /* The launch between the run's two timing events: hs_last_run_ms brackets the kernel alone, so every other piece of
  * host work (function attributes, uploads, memsets) is issued before this call.  `info` is the launch's geometry
- * (grid, block, smem) and what hs_last_launch reports of it. */
-template <typename Kernel, typename... Args>
-static int timed_launch(hs_engine *E, const hs_launch_info &info, Kernel kern, Args... args)
+ * (grid, block, smem) and what hs_last_launch reports of it; `kern` is entry info.flags of the kernel's table.
+ * cudaLaunchKernel does not check `args` against the kernel's parameters: each launcher builds its array next to its
+ * table, and the instantiations of one kernel differ only in the last parameter, whose type the flag word's bucket
+ * bits give (bucket_arg). */
+static int timed_launch(hs_engine *E, const hs_launch_info &info, const void *kern, void **args)
 {
     CUDA_TRY(cudaEventRecord(E->ev0, E->stream));
-    kern<<<info.grid, info.block, info.smem, E->stream>>>(args...);
-    CUDA_TRY(cudaGetLastError());
+    (void)cudaLaunchKernel(kern, dim3(info.grid), dim3(info.block), args, info.smem, E->stream);   /* what <<<>>> calls */
+    CUDA_TRY(cudaGetLastError());                    /* reports the launch's error and clears it, as after <<<>>> */
     CUDA_TRY(cudaEventRecord(E->ev1, E->stream));
     E->launches += 1;
     E->last_launch = info;
     return HS_OK;
 }
-
-#define HS_K4(K, F) K<F>, K<F + 1>, K<F + 2>, K<F + 3>
 
 static int launch_lane(hs_engine *E, const hs_kernel_run &R, const hs_kernel_out &O, bool want_hash, bool want_rec,
                        const hs_bucket_pct_args &BK)
@@ -372,40 +392,27 @@ static int launch_lane(hs_engine *E, const hs_kernel_run &R, const hs_kernel_out
     const int fl = (want_hash ? HS_LF_HASH : 0) | (want_rec ? HS_LF_REC : 0) |
                    (M.has_profile ? HS_LF_PROFILE : 0) | (simple ? HS_LF_SIMPLE : 0) | (buckets ? HS_LF_BUCKETS : 0) |
                    (pct ? HS_LF_BUCKET_PCT : 0);
-    using kernel = void (*)(hs_lane_model, hs_kernel_run, hs_lane_state *, hs_ring_entry *, hs_cont *, hs_kernel_out, hs_no_bucket_args);
-    using bucket_kernel = void (*)(hs_lane_model, hs_kernel_run, hs_lane_state *, hs_ring_entry *, hs_cont *, hs_kernel_out, hs_bucket_args);
-    using pct_kernel = void (*)(hs_lane_model, hs_kernel_run, hs_lane_state *, hs_ring_entry *, hs_cont *, hs_kernel_out, hs_bucket_pct_args);
-    static const kernel kernels[] = {HS_K4(hs_lane_kernel, 0), HS_K4(hs_lane_kernel, 4),     /* fl <= 11: the SIMPLE */
-                                     HS_K4(hs_lane_kernel, 8)};                               /* model has no profile */
-    /* [HASH | PROFILE ? 2 : 0 | SIMPLE ? 4 : 0] */
-    static const bucket_kernel bucket_kernels[] = {hs_lane_kernel<HS_LF_BUCKETS>, hs_lane_kernel<HS_LF_BUCKETS | HS_LF_HASH>,
-                                            hs_lane_kernel<HS_LF_BUCKETS | HS_LF_PROFILE>, hs_lane_kernel<HS_LF_BUCKETS | HS_LF_PROFILE | HS_LF_HASH>,
-                                            hs_lane_kernel<HS_LF_BUCKETS | HS_LF_SIMPLE>, hs_lane_kernel<HS_LF_BUCKETS | HS_LF_SIMPLE | HS_LF_HASH>};
-    /* with percentiles, the same order */
-#define HS_LP_(F) hs_lane_kernel<HS_LF_BUCKETS | HS_LF_BUCKET_PCT | (F)>
-    static const pct_kernel pct_kernels[] = {HS_LP_(0), HS_LP_(HS_LF_HASH), HS_LP_(HS_LF_PROFILE), HS_LP_(HS_LF_PROFILE | HS_LF_HASH),
-                                             HS_LP_(HS_LF_SIMPLE), HS_LP_(HS_LF_SIMPLE | HS_LF_HASH)};
-#undef HS_LP_
+    static const auto kernels = kernel_table<64>([](auto f) -> const void * {
+        if constexpr (hs_lane_built(f)) return (const void *)hs_lane_kernel<f>;
+        return nullptr;
+    });
+    hs_lane_state *states = (hs_lane_state *)E->d_state.p;
+    hs_ring_entry *rings = (hs_ring_entry *)E->d_rings.p;
+    hs_cont *conts = (hs_cont *)E->d_conts.p;
+    void *args[] = {(void *)&M, (void *)&R, &states, &rings, &conts, (void *)&O, bucket_arg(BK, buckets, pct)};
+    if (!kernels[fl]) return fail(HS_ERR_INVALID, "the lane engine has no kernel for flag word %d", fl);
     const hs_launch_info info = {2, HS_KERNEL_LANE, (uint32_t)fl, 1, 0, (n + HS_LANE_THREADS - 1) / HS_LANE_THREADS,
                                  HS_LANE_THREADS, 0};
-    const uint32_t bi = (fl & HS_LF_HASH) | (M.has_profile ? 2 : 0) | (simple ? 4 : 0);
-    if (pct)
-        return timed_launch(E, info, pct_kernels[bi], M, R, (hs_lane_state *)E->d_state.p, (hs_ring_entry *)E->d_rings.p,
-                            (hs_cont *)E->d_conts.p, O, BK);
-    if (buckets)
-        return timed_launch(E, info, bucket_kernels[bi], M, R, (hs_lane_state *)E->d_state.p, (hs_ring_entry *)E->d_rings.p,
-                            (hs_cont *)E->d_conts.p, O, (const hs_bucket_args &)BK);
-    return timed_launch(E, info, kernels[fl], M, R, (hs_lane_state *)E->d_state.p, (hs_ring_entry *)E->d_rings.p,
-                        (hs_cont *)E->d_conts.p, O, hs_no_bucket_args());
+    return timed_launch(E, info, kernels[fl], args);
 }
 
 static const uint32_t HS_WARP_SMEM_MAX = 227 * 1024 - 1024;      /* dynamic shared memory of a warp-engine CTA */
 
 /* What the warp and the thread engine share: the future-event slots, the servers' queue-ring indices, the replica
- * state and queue-ring buffers, and the model flags (*fl).  A bucketed run (BK->n != 0) appends the rows' time-bucket
- * accumulators to the replica block and sets BK->acc_off to their offset. */
+ * state and queue-ring buffers, and the flags of the model and the run (*fl).  A bucketed run (BK->n != 0) appends the
+ * rows' time-bucket accumulators to the replica block and sets BK->acc_off to their offset. */
 static int general_setup(hs_engine *E, const hs_kernel_run &R, bool thread, bool want_hash, bool want_rec,
-                         hs_warp_model &M, int *fl, hs_bucket_args *BK)
+                         hs_warp_model &M, int *fl, hs_bucket_pct_args *BK)
 {
     const uint32_t n = R.n_replicas;
     const uint32_t ne = (uint32_t)E->ents.size();
@@ -460,10 +467,12 @@ static int general_setup(hs_engine *E, const hs_kernel_run &R, bool thread, bool
     M.n_backends = (uint32_t)E->backends.size(); M.model_bytes = 0;
     M.outbox_cap = E->outbox_cap; M.inbox_cap = E->inbox_cap;
     M.fixed_slots = 0; M.n_faults = n_faults;
-    /* a model with faults runs the FAULTS instantiations, which always include the profile path (half the kernels to
-     * build; with no profile row it is one untaken branch per tick) */
-    *fl = (want_hash ? HS_WF_HASH : 0) | (want_rec ? HS_WF_REC : 0) | (any_profile || n_faults ? HS_WF_PROFILE : 0) |
-          (n_faults ? HS_WF_FAULTS : 0);
+    /* a model with faults runs the FAULTS instantiations and a bucketed run the BUCKETS ones (never with the recorder:
+     * hs_run refuses that combination), which always include the profile path (half the kernels to build; with no
+     * profile row it is one untaken branch per tick) */
+    const bool buckets = BK->n != 0;
+    *fl = (want_hash ? HS_WF_HASH : 0) | (want_rec ? HS_WF_REC : 0) | (any_profile || n_faults || buckets ? HS_WF_PROFILE : 0) |
+          (n_faults ? HS_WF_FAULTS : 0) | (buckets ? HS_WF_BUCKETS : 0) | (buckets && BK->cap ? HS_WF_BUCKET_PCT : 0);
     return HS_OK;
 }
 
@@ -487,38 +496,19 @@ static int launch_warp(hs_engine *E, const hs_kernel_run &R, const hs_kernel_out
     const uint32_t grid = std::min<uint32_t>((R.n_replicas + warps - 1) / warps, (uint32_t)E->sm_count * blocks_per_sm);
     if ((rc = E->d_counter.ensure(16))) return rc;
     CUDA_TRY(cudaMemsetAsync(E->d_counter.p, 0, 16, E->stream));
-    using kernel = void (*)(hs_warp_model, hs_kernel_run, unsigned char *, hs_wring_entry *, hs_kernel_out, unsigned int *, hs_no_bucket_args);
-    using bucket_kernel = void (*)(hs_warp_model, hs_kernel_run, unsigned char *, hs_wring_entry *, hs_kernel_out, unsigned int *, hs_bucket_args);
-    using pct_kernel = void (*)(hs_warp_model, hs_kernel_run, unsigned char *, hs_wring_entry *, hs_kernel_out, unsigned int *, hs_bucket_pct_args);
-    static const kernel kernels[] = {HS_K4(hs_warp_kernel, 0), HS_K4(hs_warp_kernel, 4)};
-    static const kernel fault_kernels[] = {HS_K4(hs_warp_kernel, HS_WF_FAULTS | HS_WF_PROFILE)};
-    /* time buckets (never with the recorder): [HASH | FAULTS ? 2 : 0], the profile path always compiled in */
-    static const bucket_kernel bucket_kernels[] = {hs_warp_kernel<HS_WF_BUCKETS | HS_WF_PROFILE>, hs_warp_kernel<HS_WF_BUCKETS | HS_WF_PROFILE | HS_WF_HASH>,
-                                            hs_warp_kernel<HS_WF_BUCKETS | HS_WF_FAULTS | HS_WF_PROFILE>,
-                                            hs_warp_kernel<HS_WF_BUCKETS | HS_WF_FAULTS | HS_WF_PROFILE | HS_WF_HASH>};
-    /* with percentiles, the same order */
-#define HS_WP_(F) hs_warp_kernel<HS_WF_BUCKETS | HS_WF_BUCKET_PCT | HS_WF_PROFILE | (F)>
-    static const pct_kernel pct_kernels[] = {HS_WP_(0), HS_WP_(HS_WF_HASH), HS_WP_(HS_WF_FAULTS), HS_WP_(HS_WF_FAULTS | HS_WF_HASH)};
-#undef HS_WP_
-    const bool pct = BK.n && BK.cap;
-    const hs_launch_info info = {1, HS_KERNEL_WARP, (uint32_t)(fl | (BK.n ? HS_WF_BUCKETS | HS_WF_PROFILE : 0) | (pct ? HS_WF_BUCKET_PCT : 0)),
-                                 1, 0, grid, warps * 32, smem};
-    const uint32_t bi = (fl & HS_WF_HASH) | ((fl & HS_WF_FAULTS) ? 2 : 0);
-    if (pct) {
-        CUDA_TRY(cudaFuncSetAttribute(pct_kernels[bi], cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
-        return timed_launch(E, info, pct_kernels[bi], M, R, (unsigned char *)E->d_state.p, (hs_wring_entry *)E->d_rings.p, O,
-                            (unsigned int *)E->d_counter.p, BK);
-    }
-    if (BK.n) {
-        const bucket_kernel kern = bucket_kernels[bi];
-        CUDA_TRY(cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
-        return timed_launch(E, info, kern, M, R, (unsigned char *)E->d_state.p, (hs_wring_entry *)E->d_rings.p, O,
-                            (unsigned int *)E->d_counter.p, (const hs_bucket_args &)BK);
-    }
-    const kernel kern = (fl & HS_WF_FAULTS) ? fault_kernels[fl & 3] : kernels[fl];
-    CUDA_TRY(cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
-    return timed_launch(E, info, kern, M, R, (unsigned char *)E->d_state.p,
-                        (hs_wring_entry *)E->d_rings.p, O, (unsigned int *)E->d_counter.p, hs_no_bucket_args());
+    static const auto kernels = kernel_table<256>([](auto f) -> const void * {
+        if constexpr (hs_warp_built(f)) return (const void *)hs_warp_kernel<f>;
+        return nullptr;
+    });
+    unsigned char *blocks = (unsigned char *)E->d_state.p;
+    hs_wring_entry *rings = (hs_wring_entry *)E->d_rings.p;
+    unsigned int *next_replica = (unsigned int *)E->d_counter.p;
+    void *args[] = {&M, (void *)&R, &blocks, &rings, (void *)&O, &next_replica,
+                    bucket_arg(BK, fl & HS_WF_BUCKETS, fl & HS_WF_BUCKET_PCT)};
+    if (!kernels[fl]) return fail(HS_ERR_INVALID, "the warp engine has no kernel for flag word %d", fl);
+    CUDA_TRY(cudaFuncSetAttribute(kernels[fl], cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
+    const hs_launch_info info = {1, HS_KERNEL_WARP, (uint32_t)fl, 1, 0, grid, warps * 32, smem};
+    return timed_launch(E, info, kernels[fl], args);
 }
 
 static int launch_thread(hs_engine *E, hs_kernel_run R, const hs_kernel_out &O, bool want_hash, bool want_rec, bool linked,
@@ -552,63 +542,27 @@ static int launch_thread(hs_engine *E, hs_kernel_run R, const hs_kernel_out &O, 
     while (total + level <= budget && total + level <= S) { total += level; level *= HS_T_ARITY; top = total; }
     R.heap_top = (top < 1 + HS_T_ARITY || R.lane_stride == 32) ? 0 : top;  /* one replica per warp: its heap sits in L1 anyway */
     const size_t dyn_smem = (size_t)(HS_T_KS * 3u + R.heap_top) * rpb * 16;
-    using kernel = void (*)(hs_warp_model, hs_kernel_run, unsigned char *, hs_wring_entry *, hs_kernel_out);
-    using bucket_kernel = void (*)(hs_warp_model, hs_kernel_run, unsigned char *, hs_wring_entry *, hs_kernel_out, hs_bucket_args);
-    using pct_kernel = void (*)(hs_warp_model, hs_kernel_run, unsigned char *, hs_wring_entry *, hs_kernel_out, hs_bucket_pct_args);
-    static const kernel kernels[] = {HS_K4(hs_thread_kernel, 0), HS_K4(hs_thread_kernel, 4), HS_K4(hs_thread_kernel, 8),
-                                     HS_K4(hs_thread_kernel, 12), HS_K4(hs_thread_kernel, 16), HS_K4(hs_thread_kernel, 20),
-                                     HS_K4(hs_thread_kernel, 24), HS_K4(hs_thread_kernel, 28)};
-    static const kernel wide_kernels[] = {HS_K4(hs_thread_kernel_wide, 0), HS_K4(hs_thread_kernel_wide, 4)};
-    /* [fl & 3 | HEAPTOP ? 4 : 0 | LINKED ? 8 : 0]: linked launches never take the wide kernel, so it has no linked form */
-    static const kernel fault_kernels[] = {HS_K4(hs_thread_kernel, HS_WF_FAULTS | HS_WF_PROFILE),
-                                           HS_K4(hs_thread_kernel, HS_WF_FAULTS | HS_WF_HEAPTOP | HS_WF_PROFILE),
-                                           HS_K4(hs_thread_kernel, HS_WF_LINKED | HS_WF_FAULTS | HS_WF_PROFILE),
-                                           HS_K4(hs_thread_kernel, HS_WF_LINKED | HS_WF_FAULTS | HS_WF_HEAPTOP | HS_WF_PROFILE)};
-    static const kernel fault_wide_kernels[] = {HS_K4(hs_thread_kernel_wide, HS_WF_FAULTS | HS_WF_PROFILE)};
-    /* time buckets (never with the recorder), the profile path always compiled in:
-     * [HASH | HEAPTOP ? 2 : 0 | FAULTS ? 4 : 0 | LINKED ? 8 : 0] and, wide (never linked), [HASH | FAULTS ? 2 : 0] */
-#define HS_TB_(F) hs_thread_bucket_kernel<HS_WF_BUCKETS | HS_WF_PROFILE | (F)>
-#define HS_TB8_(L) HS_TB_(L), HS_TB_((L) | HS_WF_HASH), HS_TB_((L) | HS_WF_HEAPTOP), HS_TB_((L) | HS_WF_HEAPTOP | HS_WF_HASH),         \
-                   HS_TB_((L) | HS_WF_FAULTS), HS_TB_((L) | HS_WF_FAULTS | HS_WF_HASH),                                               \
-                   HS_TB_((L) | HS_WF_FAULTS | HS_WF_HEAPTOP), HS_TB_((L) | HS_WF_FAULTS | HS_WF_HEAPTOP | HS_WF_HASH)
-    static const bucket_kernel bucket_kernels[] = {HS_TB8_(0), HS_TB8_(HS_WF_LINKED)};
-#undef HS_TB8_
-#undef HS_TB_
-#define HS_TBW_(F) hs_thread_bucket_kernel_wide<HS_WF_BUCKETS | HS_WF_PROFILE | (F)>
-    static const bucket_kernel bucket_wide_kernels[] = {HS_TBW_(0), HS_TBW_(HS_WF_HASH), HS_TBW_(HS_WF_FAULTS), HS_TBW_(HS_WF_FAULTS | HS_WF_HASH)};
-#undef HS_TBW_
-    /* with percentiles, the same order */
-#define HS_TP_(F) hs_thread_bucket_kernel<HS_WF_BUCKETS | HS_WF_BUCKET_PCT | HS_WF_PROFILE | (F)>
-#define HS_TP8_(L) HS_TP_(L), HS_TP_((L) | HS_WF_HASH), HS_TP_((L) | HS_WF_HEAPTOP), HS_TP_((L) | HS_WF_HEAPTOP | HS_WF_HASH),         \
-                   HS_TP_((L) | HS_WF_FAULTS), HS_TP_((L) | HS_WF_FAULTS | HS_WF_HASH),                                               \
-                   HS_TP_((L) | HS_WF_FAULTS | HS_WF_HEAPTOP), HS_TP_((L) | HS_WF_FAULTS | HS_WF_HEAPTOP | HS_WF_HASH)
-    static const pct_kernel pct_kernels[] = {HS_TP8_(0), HS_TP8_(HS_WF_LINKED)};
-#undef HS_TP8_
-#undef HS_TP_
-#define HS_TPW_(F) hs_thread_bucket_kernel_wide<HS_WF_BUCKETS | HS_WF_BUCKET_PCT | HS_WF_PROFILE | (F)>
-    static const pct_kernel pct_wide_kernels[] = {HS_TPW_(0), HS_TPW_(HS_WF_HASH), HS_TPW_(HS_WF_FAULTS), HS_TPW_(HS_WF_FAULTS | HS_WF_HASH)};
-#undef HS_TPW_
-    if (BK.n) fl |= HS_WF_BUCKETS | HS_WF_PROFILE | (BK.cap ? HS_WF_BUCKET_PCT : 0);
     /* small launches (every block resident at 4 blocks per SM, no shared-memory heap top, not linked): the spill-free
      * instantiation, see hs_thread_kernel_wide */
     const bool wide = !R.heap_top && !linked && tblocks <= (uint32_t)E->sm_count * HS_T_WIDE_BLOCKS;
     if (!wide) fl |= (R.heap_top ? HS_WF_HEAPTOP : 0) | (linked ? HS_WF_LINKED : 0);
+    static const auto kernels = kernel_table<256>([](auto f) -> const void * {
+        if constexpr (hs_thread_built(f)) return (const void *)hs_thread_kernel<f>;
+        return nullptr;
+    });
+    static const auto wide_kernels = kernel_table<256>([](auto f) -> const void * {
+        if constexpr (hs_thread_wide_built(f)) return (const void *)hs_thread_kernel_wide<f>;
+        return nullptr;
+    });
+    unsigned char *blocks = (unsigned char *)E->d_state.p;
+    hs_wring_entry *rings = (hs_wring_entry *)E->d_rings.p;
+    void *args[] = {&M, &R, &blocks, &rings, (void *)&O, bucket_arg(BK, fl & HS_WF_BUCKETS, fl & HS_WF_BUCKET_PCT)};
+    const void *kern = (wide ? wide_kernels : kernels)[fl];
+    if (!kern) return fail(HS_ERR_INVALID, "the thread engine has no %skernel for flag word %d", wide ? "wide " : "", fl);
     const hs_launch_info info = {3, wide ? (uint32_t)HS_KERNEL_THREAD_WIDE : (uint32_t)HS_KERNEL_THREAD, (uint32_t)fl,
                                  R.lane_stride, R.heap_top, tblocks, HS_THREAD_BLOCK, (uint32_t)dyn_smem};
-    const uint32_t bi = (fl & HS_WF_HASH) | ((fl & HS_WF_HEAPTOP) ? 2 : 0) | ((fl & HS_WF_FAULTS) ? 4 : 0) | ((fl & HS_WF_LINKED) ? 8 : 0);
-    const uint32_t wbi = (fl & HS_WF_HASH) | ((fl & HS_WF_FAULTS) ? 2 : 0);
-    if (fl & HS_WF_BUCKET_PCT)
-        return timed_launch(E, info, wide ? pct_wide_kernels[wbi] : pct_kernels[bi], M, R, (unsigned char *)E->d_state.p,
-                            (hs_wring_entry *)E->d_rings.p, O, BK);
-    if (fl & HS_WF_BUCKETS)
-        return timed_launch(E, info, wide ? bucket_wide_kernels[wbi] : bucket_kernels[bi], M, R, (unsigned char *)E->d_state.p,
-                            (hs_wring_entry *)E->d_rings.p, O, (const hs_bucket_args &)BK);
-    const kernel kern = !(fl & HS_WF_FAULTS) ? (wide ? wide_kernels[fl] : kernels[fl])
-                      : wide ? fault_wide_kernels[fl & 3]
-                      : fault_kernels[(fl & 3) | ((fl & HS_WF_HEAPTOP) ? 4 : 0) | ((fl & HS_WF_LINKED) ? 8 : 0)];
-    return timed_launch(E, info, kern, M, R, (unsigned char *)E->d_state.p, (hs_wring_entry *)E->d_rings.p, O);
+    return timed_launch(E, info, kern, args);
 }
-#undef HS_K4
 
 /* The per-cell reduction of the last run's bucket data `src` into `out` [n_cells][rows][n + 1] of T (hs_bucket_total
  * or hs_bucket_pct_total): the two fixed-order stages of hs_buckets.cuh over the same slices. */

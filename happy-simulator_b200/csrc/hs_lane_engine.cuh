@@ -82,6 +82,14 @@
                              without HS_LF_REC only */
 #define HS_LF_BUCKET_PCT 32 /* with HS_LF_BUCKETS: the buckets' p50 / p99 (hs_set_bucket_percentiles) */
 
+/* The flag words (F < 64) hs_lane_kernel is built for (hs_engine.cu launches it through a table indexed by the flag
+ * word): a SIMPLE model has no profile, BUCKETS never comes with the recorder, BUCKET_PCT only with BUCKETS. */
+constexpr bool hs_lane_built(int F)
+{
+    return !((F & HS_LF_SIMPLE) && (F & HS_LF_PROFILE)) && !((F & HS_LF_BUCKETS) && (F & HS_LF_REC)) &&
+           (!(F & HS_LF_BUCKET_PCT) || (F & HS_LF_BUCKETS));
+}
+
 struct hs_now_ev {        /* an event created at the current timestamp       */
     uint64_t idx;         /* Event._sort_index                               */
     int64_t created;      /* context["created_at"]                           */

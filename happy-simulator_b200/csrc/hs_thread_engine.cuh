@@ -820,42 +820,32 @@ hs_thread_body(const hs_warp_model &M, const hs_kernel_run &P, unsigned char *__
  * spills ~130 bytes per thread to get there.  hs_thread_kernel_wide: the same code with the registers it asks for (~208,
  * no spills) at 4 blocks per SM, for launches whose blocks all fit at that occupancy (small ensembles, one replica per
  * warp): every spill reload sits on the one dependent-instruction chain a warp has there.  configs[3] at one GPU's 1 024
- * replicas: 1.125e9 -> 1.25e9 events/s; at 16 384 replicas of configs[2] the wide form would lose a quarter (second wave). */
+ * replicas: 1.125e9 -> 1.25e9 events/s; at 16 384 replicas of configs[2] the wide form would lose a quarter (second wave).
+ * Both take the bucket arguments last, as the lane and warp kernels do: hs_bucket_args with HS_WF_BUCKETS,
+ * hs_bucket_pct_args with HS_WF_BUCKET_PCT, the empty hs_no_bucket_args otherwise. */
 template <int FLAGS>
 __global__ void __launch_bounds__(HS_THREAD_BLOCK, HS_T_MINBLOCKS)
 hs_thread_kernel(hs_warp_model M, hs_kernel_run P, unsigned char *__restrict__ blocks,
-                 hs_wring_entry *__restrict__ rings, hs_kernel_out O)
+                 hs_wring_entry *__restrict__ rings, hs_kernel_out O,
+                 typename hs_bucket_args_of<(FLAGS & HS_WF_BUCKETS) != 0, (FLAGS & HS_WF_BUCKET_PCT) != 0>::type BK)
 {
-    hs_thread_body<FLAGS>(M, P, blocks, rings, O, hs_no_bucket_args());
+    hs_thread_body<FLAGS>(M, P, blocks, rings, O, BK);
 }
 
 #define HS_T_WIDE_BLOCKS 4
 template <int FLAGS>
 __global__ void __launch_bounds__(HS_THREAD_BLOCK, HS_T_WIDE_BLOCKS)
 hs_thread_kernel_wide(hs_warp_model M, hs_kernel_run P, unsigned char *__restrict__ blocks,
-                      hs_wring_entry *__restrict__ rings, hs_kernel_out O)
-{
-    hs_thread_body<FLAGS>(M, P, blocks, rings, O, hs_no_bucket_args());
-}
-
-/* the same two entry points for the time-bucket instantiations (FLAGS with HS_WF_BUCKETS): the bucket arguments come
- * as one more parameter, which the kernels above do not have (hs_bucket_pct_args with HS_WF_BUCKET_PCT) */
-template <int FLAGS>
-__global__ void __launch_bounds__(HS_THREAD_BLOCK, HS_T_MINBLOCKS)
-hs_thread_bucket_kernel(hs_warp_model M, hs_kernel_run P, unsigned char *__restrict__ blocks,
-                        hs_wring_entry *__restrict__ rings, hs_kernel_out O,
-                        typename hs_bucket_args_of<true, (FLAGS & HS_WF_BUCKET_PCT) != 0>::type BK)
+                      hs_wring_entry *__restrict__ rings, hs_kernel_out O,
+                      typename hs_bucket_args_of<(FLAGS & HS_WF_BUCKETS) != 0, (FLAGS & HS_WF_BUCKET_PCT) != 0>::type BK)
 {
     hs_thread_body<FLAGS>(M, P, blocks, rings, O, BK);
 }
 
-template <int FLAGS>
-__global__ void __launch_bounds__(HS_THREAD_BLOCK, HS_T_WIDE_BLOCKS)
-hs_thread_bucket_kernel_wide(hs_warp_model M, hs_kernel_run P, unsigned char *__restrict__ blocks,
-                             hs_wring_entry *__restrict__ rings, hs_kernel_out O,
-                             typename hs_bucket_args_of<true, (FLAGS & HS_WF_BUCKET_PCT) != 0>::type BK)
-{
-    hs_thread_body<FLAGS>(M, P, blocks, rings, O, BK);
-}
+/* The flag words each entry point is built for (hs_engine.cu launches through a table of them): the general engines'
+ * set, and the wide kernel never with HS_WF_HEAPTOP (it is for launches without a heap top) or HS_WF_LINKED (linked
+ * launches never take it). */
+constexpr bool hs_thread_built(int F) { return hs_general_built(F); }
+constexpr bool hs_thread_wide_built(int F) { return hs_general_built(F) && !(F & (HS_WF_HEAPTOP | HS_WF_LINKED)); }
 
 #endif /* HS_THREAD_ENGINE_CUH */

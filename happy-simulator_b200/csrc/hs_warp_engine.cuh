@@ -46,6 +46,17 @@
                               other launch.  The row of a SINK / PROBE entity is the low word of its device row's d1 */
 #define HS_WF_BUCKET_PCT 128 /* with HS_WF_BUCKETS: the buckets' p50 / p99 (hs_set_bucket_percentiles) */
 
+/* The flag words (F < 256) the general engines are built for: FAULTS and BUCKETS always with the profile path (half the
+ * kernels to build), BUCKETS never with the recorder, BUCKET_PCT only with BUCKETS.  hs_warp_kernel has none of the
+ * thread-engine flags (hs_engine.cu launches it through a table indexed by the flag word; the thread engine's
+ * predicates are next to its kernels). */
+constexpr bool hs_general_built(int F)
+{
+    return (!(F & HS_WF_FAULTS) || (F & HS_WF_PROFILE)) && (!(F & HS_WF_BUCKETS) || ((F & HS_WF_PROFILE) && !(F & HS_WF_REC))) &&
+           (!(F & HS_WF_BUCKET_PCT) || (F & HS_WF_BUCKETS));
+}
+constexpr bool hs_warp_built(int F) { return hs_general_built(F) && !(F & (HS_WF_HEAPTOP | HS_WF_LINKED)); }
+
 struct __align__(16) hs_warp_hdr {      /* 128 B */
     int64_t now; uint64_t ctr; int64_t processed; uint64_t hash;
     int64_t n_smp, n_svc;
