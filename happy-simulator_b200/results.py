@@ -7,6 +7,8 @@ import sys
 from dataclasses import dataclass, field
 from typing import Any
 
+import numpy as np
+
 from . import _abi as A
 from . import sketching
 
@@ -45,10 +47,32 @@ class SimulationSummary:
                 "entities": {k: vars(v) for k, v in self.entities.items()}}
 
 
+def _dropped_sink_requests(model, rec):
+    """Mask of the REQ_SINK records aimed at a sink that a node fault had crashed or paused when the event was popped.
+    The engines record and count such an event, but Event.invoke drops it (core/event.py:261-262): it leaves no sample.
+    The crashed flag at each record is the set / clear of the last FAULT record of that sink before it."""
+    dropped = np.zeros(len(rec), bool)
+    fr = model.ids_of(A.HS_ENT_FAULT)
+    if not len(fr):
+        return dropped
+    E = model.entities
+    fpos = np.flatnonzero(rec["kind"] == A.HS_EV_FAULT)
+    frow = rec["entity"][fpos]
+    ftgt, fset = E["target"][frow], E["i1"][frow]
+    req = np.flatnonzero(rec["kind"] == A.HS_EV_REQ_SINK)
+    for s in np.unique(ftgt):
+        p, v = fpos[ftgt == s], fset[ftgt == s]
+        q = req[rec["entity"][req] == s]
+        k = np.searchsorted(p, q) - 1              # the sink's last FAULT record before each request
+        dropped[q[k >= 0]] = v[k[k >= 0]] != 0
+    return dropped
+
+
 def demultiplex(model, out, r: int):
     """Replica ``r``'s Sink samples and service times per entity row: ({sink or probe row: samples, None if none were
     recorded}, {server row: [float]}).  One collector (server) takes the whole stream; several are told apart by the
-    entity of each REQ_SINK / PROBE (REQ_WORKER) event record, in stream order."""
+    entity of each REQ_SINK / PROBE (REQ_WORKER) event record, in stream order, leaving out the requests a crashed sink
+    dropped."""
     s = out["summaries"][r]
     sinks = model.ids_of(A.HS_ENT_SINK) + model.ids_of(A.HS_ENT_PROBE)
     servers = model.ids_of(A.HS_ENT_SERVER)
@@ -60,7 +84,8 @@ def demultiplex(model, out, r: int):
         if len(sinks) == 1:
             per_sink[sinks[0]] = samples
         elif rec is not None:
-            who = rec["entity"][(rec["kind"] == A.HS_EV_REQ_SINK) | (rec["kind"] == A.HS_EV_PROBE)][: len(samples)]
+            sel = ((rec["kind"] == A.HS_EV_REQ_SINK) | (rec["kind"] == A.HS_EV_PROBE)) & ~_dropped_sink_requests(model, rec)
+            who = rec["entity"][sel][: len(samples)]
             for i in sinks:
                 per_sink[i] = samples[who == i]
     if out.get("service_samples") is not None:

@@ -118,14 +118,17 @@ def cases():
     return c
 
 
-def run_case(model, build_schedule, kw):
+def build_case(model, build_schedule, kw):
+    """The reference's Simulation of a case, built and not run: (harness context, Simulation, FaultSchedule, the
+    lowering.fault_events of the schedule, the model plus its FAULT rows)"""
     RH._import_reference()
     from happysimulator import faults as F
     from happysimulator.core.simulation import Simulation
     from happysimulator.core.temporal import Instant
     end_ns = int(kw["end_s"] * 1e9)
     ctx = RH.run_reference(model, seed=kw["seed"], rid=kw["rid"], end_ns=end_ns, chash_vnodes=kw.get("chash_vnodes"),
-                           sketch_seeds=kw.get("sketch_seeds"), zipf_s=kw.get("zipf_s"), _build_only=True)
+                           sketch_seeds=kw.get("sketch_seeds"), zipf_s=kw.get("zipf_s"),
+                           profile_objects=kw.get("profile_objects"), _build_only=True)
     objs = ctx["objs"]
     schedule = build_schedule({getattr(o, "name", None): o for o in objs}, F)
     handles = list(schedule._handles)
@@ -140,6 +143,12 @@ def run_case(model, build_schedule, kw):
             for tgt, t_ns, crash, idx, ev in fev]
     fm = dataclasses.replace(model, entities=np.concatenate([model.entities, np.array(rows, dtype=A.ENTITY_DTYPE)]),
                              names=list(model.names) + [f"fault:{tgt.name}" for tgt, *_ in fev])
+    return ctx, sim, schedule, fev, fm
+
+
+def run_case(model, build_schedule, kw):
+    ctx, sim, schedule, fev, fm = build_case(model, build_schedule, kw)
+    objs = ctx["objs"]
     row_of = {id(ev): model.n_entities + k for k, (*_, ev) in enumerate(fev)}
     fired = {i: 0 for i in row_of.values()}
     cancelled = {i: 0 for i in row_of.values()}
@@ -198,7 +207,7 @@ def run_case(model, build_schedule, kw):
     meta = dict(kw, crashed=crashed, events_cancelled=np.array(summary.events_cancelled, dtype=np.int64),
                 fault_stats=np.array([fstats.faults_scheduled, fstats.faults_activated, fstats.faults_deactivated,
                                       fstats.faults_cancelled], dtype=np.int64))
-    meta.pop("cancel", None); meta.pop("expect_tie", None); meta.pop("chash_vnodes", None)
+    meta.pop("cancel", None); meta.pop("expect_tie", None); meta.pop("chash_vnodes", None); meta.pop("profile_objects", None)
     return fm, ref, meta
 
 

@@ -196,6 +196,90 @@ def random_model_v2(seed: int, with_extras: bool = False):
     return (model, end_s, what, extras) if with_extras else (model, end_s, what)
 
 
+FAULT_SEED_OFFSET, FAULT_SEED_OFFSET_V2 = 1000, 5000
+
+
+def random_fault_plan(model, end_s: float, seed: int, offset: int = FAULT_SEED_OFFSET):
+    """A random node-fault schedule for ``model``: 1 to 4 faults (crash, crash with restart, pause) on entities other
+    than probes and their tick sources, at times in [0, end_s] rounded to the millisecond, each cancelled with
+    probability 0.2.  -> (plan: [(kind, entity name, a_s, b_s)], indices of the cancelled faults)"""
+    import random
+    rng = random.Random(offset + seed)
+    ents = model.entities
+    names = [n for i, n in enumerate(model.names) if int(ents["kind"][i]) != A.HS_ENT_PROBE and not (
+        int(ents["kind"][i]) == A.HS_ENT_SOURCE and int(ents["kind"][int(ents["target"][i])]) == A.HS_ENT_PROBE)]
+    plan = []
+    for _ in range(rng.randint(1, 4)):
+        nm = rng.choice(names)
+        a = round(rng.uniform(0.0, end_s), 3)
+        kind = rng.choice(["crash", "crash_restart", "pause"])
+        b = round(a + rng.uniform(0.01, end_s / 2), 3)
+        plan.append((kind, nm, a, b))
+    cancel = [k for k in range(len(plan)) if rng.random() < 0.2]
+    return plan, cancel
+
+
+def _fault_seeds_v1(n=60):
+    """the first n seeds of random_model whose model the reference harness can build (no random key table)"""
+    out, s = [], 0
+    while len(out) < n:
+        if not random_model(s, with_extras=True)[3]["random_key_table"]:
+            out.append(s)
+        s += 1
+    return out
+
+
+FAULT_SEEDS_V1 = _fault_seeds_v1()          # against the reference (CPU) and tests/golden/random_fault_models.npz
+FAULT_SEEDS_V2 = list(range(60))
+
+
+def random_fault_case(version: int, seed: int, scale: float = 1.0):
+    """A seeded random model (random_model or random_model_v2) with its random fault plan, drawn on the model's
+    horizon times ``scale`` (a shorter run keeps its faults).
+    -> (FlatModel without FAULT rows, end_seconds, plan, cancel, run seed, description, extras for the harness)"""
+    if version == 1:
+        model, end_s, what, ex = random_model(seed, with_extras=True)
+        end_s = min(float(end_s), 6.0) * scale
+        plan, cancel = random_fault_plan(model, end_s, seed)
+        return model, end_s, plan, cancel, seed, what, ex
+    model, end_s, what, ex = random_model_v2(seed, with_extras=True)
+    end_s = float(end_s) * scale
+    plan, cancel = random_fault_plan(model, end_s, seed, FAULT_SEED_OFFSET_V2)
+    return model, end_s, plan, cancel, 2000 + seed, what, ex
+
+
+def fault_schedule(plan, F):
+    """``plan`` as a FaultSchedule of the module ``F`` (the reference's happysimulator.faults or the mirror's api)"""
+    s = F.FaultSchedule()
+    for kind, nm, a, b in plan:
+        s.add(F.CrashNode(nm, at=a) if kind == "crash" else F.CrashNode(nm, at=a, restart_at=b) if kind == "crash_restart"
+              else F.PauseNode(nm, start=a, end=b))
+    return s
+
+
+def with_faults(model, plan, cancel):
+    """``model`` plus one FAULT row per fault event of ``plan``, as lowering.fault_events lowers a FaultSchedule built
+    when the Simulation is: a crash (or pause) event and, for crash_restart and pause, a restart (resume) event, at
+    Instant.from_seconds of the plan's times; bootstrap sort indices after the sources' and probes' first ticks (one
+    SOURCE row each), one per event in schedule order.  Names resolve as FaultSchedule._build_context does, the last of
+    the entities, then the sources, winning."""
+    import dataclasses
+    ents = model.entities
+    kinds = ents["kind"]
+    order = [i for i in range(model.n_entities) if int(kinds[i]) not in (A.HS_ENT_SOURCE, A.HS_ENT_PROBE, A.HS_ENT_REMOTE)] \
+        + [i for i in range(model.n_entities) if int(kinds[i]) == A.HS_ENT_SOURCE]
+    by_name = {model.names[i]: i for i in order}
+    idx = int((kinds == A.HS_ENT_SOURCE).sum())
+    fb = hs.ModelBuilder()
+    for k, (kind, nm, a, b) in enumerate(plan):
+        for t_s, crash in [(a, True)] + ([] if kind == "crash" else [(b, False)]):
+            fb.fault(f"fault:{nm}", target=by_name[nm], time_ns=int(t_s * 1_000_000_000), crash=crash, sort_index=idx,
+                     cancelled=k in cancel)
+            idx += 1
+    return dataclasses.replace(model, entities=np.concatenate([ents, np.array(fb._rows, dtype=A.ENTITY_DTYPE)]),
+                               names=list(model.names) + fb._names)
+
+
 def random_linked_model(seed: int):
     """Random ParallelSimulation with PartitionLinks (SURVEY 8(f) row 4): 2-4 partitions, each an optional source, an
     entry (a server, a two-server chain or a load balancer over two servers), a sink and a counter; the last server of a
