@@ -287,6 +287,13 @@ static int validate_model(const hs_model_desc *m, bool partition = false)
             double d = m->cell_d0[(size_t)c * n + i]; int32_t v = m->cell_i0[(size_t)c * n + i];
             if (e.kind == HS_ENT_SOURCE && e.i3 == 0 && !(d > 0.0)) return fail(HS_ERR_INVALID, "cell %u: source rate must be > 0", c);
             if (e.kind == HS_ENT_SERVER && (v < 1 || d < 0.0)) return fail(HS_ERR_INVALID, "cell %u: bad server override", c);
+            if (e.kind == HS_ENT_CACHE_SERVER && !(d > 0.0)) return fail(HS_ERR_INVALID, "cell %u: ttl must be > 0", c);
+            if (e.kind == HS_ENT_SKETCH && e.i0 == HS_SK_TDIGEST && !(d > 0.0 && (int32_t)(d * 2.0) == e.i2))
+                return fail(HS_ERR_INVALID, "cell %u: a TDigest's compression must keep its buffer size int(compression * 2)", c);
+            /* the handlers read the i0 of LB (strategy), CachingServer (key slots), PROBE (metric) and SKETCH (algorithm)
+             * rows from the model row every cell shares, and a source's arrival kind decides its draws: only a server's
+             * i0 (its concurrency, which the replica row carries) may differ between cells.  Every row's d0 may: the
+             * handlers read it from the replica row (hs_went_init). */
             if (e.kind != HS_ENT_SERVER && v != e.i0) return fail(HS_ERR_INVALID, "cell %u: i0 override only applies to servers", c);
         }
     return HS_OK;
