@@ -71,8 +71,12 @@
 #define HS_LANE_THREADS 64
 #define HS_DRAW_BUF_SUMMARY 16  /* precomputed draws per stream per lane (even)            */
 #define HS_DRAW_BUF_RECORD 8    /* ... when the recorder staging shares the shared memory  */
+#define HS_ARR_BUF_RECORD 7     /* arrival draws per lane of the recorder kernels: 7, not 8, keeps their shared
+                                   memory at 28 160 B, at which 8 blocks of 64 threads fit an SM */
 #define HS_STAGE 16             /* staged event records per lane (recorder kernels)        */
 #define HS_FLUSH 8              /* records per flush: 8 x 16 B = one 128 B line            */
+#define HS_SMP_GROUP 4          /* Sink samples per flush: 4 x 16 B = one 64 B chunk        */
+#define HS_SVC_CHUNK 8          /* service times per chunk: 8 x 8 B = 64 B (= HS_DRAW_BUF_RECORD) */
 #define HS_LF_HASH 1      /* maintain the order hash                         */
 #define HS_LF_REC 2       /* write event records / sink / service samples    */
 #define HS_LF_PROFILE 4   /* non-constant rate profile (Simpson + Brent path) */
@@ -136,14 +140,6 @@ struct hs_lane_model {
     int32_t has_profile, pad2;        /* 0: ConstantRateProfile fast path         */
 };
 
-/* one full 32-byte sector per lane, as two back-to-back streaming 128-bit stores (STG.E.128, the widest
- * global store of sm_90a): the recorder streams are write-once per ring pass */
-__device__ __forceinline__ void hs_st256(void *p, const uint4 a, const uint4 b)
-{
-    __stcs((uint4 *)p, a);
-    __stcs((uint4 *)p + 1, b);
-}
-
 /* next arrival of a constant-rate profile, with the reference's "time travel" outcome
  * folded in: if the computed time is earlier than the current one the SourceEvent would be
  * popped and skipped and the Source never ticks again (INT64_MAX). */
@@ -166,16 +162,21 @@ hs_lane_kernel(hs_lane_model M, hs_kernel_run P, hs_lane_state *__restrict__ sta
                typename hs_bucket_args_of<(FLAGS & HS_LF_BUCKETS) != 0, (FLAGS & HS_LF_BUCKET_PCT) != 0>::type BK)
 {
     constexpr uint32_t HS_DRAW_BUF = (FLAGS & HS_LF_REC) ? HS_DRAW_BUF_RECORD : HS_DRAW_BUF_SUMMARY;
+    constexpr uint32_t ARR_BUF = (FLAGS & HS_LF_REC) ? HS_ARR_BUF_RECORD : HS_DRAW_BUF;
     constexpr uint32_t STAGE_ROWS = (FLAGS & HS_LF_REC) ? HS_STAGE : 1;
-    __shared__ int64_t sh_t[HS_DRAW_BUF][HS_LANE_THREADS];       /* arrival times A_k (ns)          */
+    static_assert(!(FLAGS & HS_LF_REC) || HS_DRAW_BUF == HS_SVC_CHUNK, "a service chunk is the whole draw buffer");
+    __shared__ int64_t sh_t[ARR_BUF][HS_LANE_THREADS];           /* arrival times A_k (ns)          */
     __shared__ double sh_svc[HS_DRAW_BUF][HS_LANE_THREADS];      /* service: Duration.to_seconds()  */
     /* recorder staging, [slot][lane]: a lane writes only its own 16-byte column, so the per-event writes do
-     * not conflict, whatever slot each lane is at.  Full 128-byte groups (8 records) are written by the whole
-     * warp, whole lines per store (the flush at the top of the loop).  Sink samples (16 B) and service
-     * times (8 B) are paired / quadrupled into one 32-byte sector per lane and store. */
+     * not conflict, whatever slot each lane is at.  Full 128-byte groups (8 records) and full 64-byte groups
+     * of Sink samples (4) are written by the whole warp at the top of the loop, several groups per store.
+     * The first three samples of a group wait in sh_smp; the fourth, which makes the group full, waits in row
+     * (st_fl - 1) % HS_STAGE of the record staging: at most 7 + 6 records are staged between two flushes,
+     * so that row is free from the sample's store to the next flush.  Service times need no staging: a
+     * whole 64-byte chunk of them is the draw buffer sh_svc itself (the refill round writes it). */
+    static_assert(HS_STAGE >= (HS_FLUSH - 1) + 6 + 1, "a free record-staging row for the fourth sample of a group");
     __shared__ __align__(16) uint4 sh_rec[STAGE_ROWS][HS_LANE_THREADS];
-    __shared__ __align__(16) uint4 sh_smp[(FLAGS & HS_LF_REC) ? HS_LANE_THREADS : 1];        /* first Sink sample of a pair */
-    __shared__ double sh_sv[(FLAGS & HS_LF_REC) ? 3 : 1][HS_LANE_THREADS];                   /* first three service times of a quad */
+    __shared__ __align__(16) uint4 sh_smp[(FLAGS & HS_LF_REC) ? HS_SMP_GROUP - 1 : 1][HS_LANE_THREADS];
     __shared__ __align__(16) hs_ring_entry sh_head[HS_LANE_THREADS];  /* next item to deliver      */
     const uint32_t tid = threadIdx.x;
     uint32_t r = blockIdx.x * blockDim.x + threadIdx.x;
@@ -241,10 +242,13 @@ hs_lane_kernel(hs_lane_model M, hs_kernel_run P, hs_lane_state *__restrict__ sta
     /* recorder staging cursors: st_wr staged, st_fl flushed; rec_pos = ring slot of record st_fl */
     const bool staged = (FLAGS & HS_LF_REC) && O.records && P.record_cap >= 2 * HS_FLUSH && (P.record_cap % HS_FLUSH) == 0;
     uint32_t st_wr = 0, st_fl = 0;
-    /* sample streams: *_sync <=> every earlier entry of the 32-byte sector being filled is staged in shared memory */
-    const bool smp_pairs = (FLAGS & HS_LF_REC) && (P.sample_cap % 2u) == 0;
-    const bool svc_quads = (FLAGS & HS_LF_REC) && (P.service_cap % 4u) == 0;
-    bool smp_sync = false, svc_sync = false;
+    /* Sink samples: smp_sync <=> every earlier entry of the 64-byte group being filled is staged; smp_full <=> a
+     * whole group is staged and waits for the next flush (its ring slots end at smp_pos) */
+    const bool smp_groups = (FLAGS & HS_LF_REC) && smp && (P.sample_cap % HS_SMP_GROUP) == 0;
+    bool smp_sync = false, smp_full = false;
+    /* Service times in 64-byte chunks, written by the refill round as the draw buffer completes one (see
+     * HS_REFILL_ROUND); other capacities are written entry by entry at the service start */
+    const bool svc_chunks = (FLAGS & HS_LF_REC) && svc_out && (P.service_cap % HS_SVC_CHUNK) == 0;
     hs_now_ev nowq[HS_NOW_CAP];
     /* the Sink's current time bucket (HS_LF_BUCKETS; an empty type otherwise): stored when it moves on and at the end */
     typename hs_bucket_acc_of<(FLAGS & HS_LF_BUCKETS) != 0>::type bacc;
@@ -281,8 +285,11 @@ hs_lane_kernel(hs_lane_model M, hs_kernel_run P, hs_lane_state *__restrict__ sta
      * provider's current_time after them; the pending SourceEvent is A_{arr_draws} = tT.
      * s_gen = service draws generated; service start number n_svc consumes draw n_svc.
      * After a pause the cursors restart at the consumed positions (a half-used Philox pair
-     * is regenerated and its first half skipped). */
-    uint64_t a_gen = arr_draws, s_gen = (uint64_t)n_svc;
+     * is regenerated and its first half skipped).  With service chunks the service cursor restarts
+     * at the start of the chunk n_svc lies in: the draws before n_svc are regenerated so that the
+     * chunk's refill finds all of it in the buffer, and rewrites the ring slots of those draws with
+     * the values an earlier launch put there; so s_gen - n_svc is negative until the first fill. */
+    uint64_t a_gen = arr_draws, s_gen = svc_chunks ? (uint64_t)n_svc & ~(uint64_t)(HS_SVC_CHUNK - 1) : (uint64_t)n_svc;
     int64_t t_gen = P.resume ? tT : 0;
 
     /* next arrival time from t (arrival_time_provider.py:66-82); a result < t would be
@@ -294,7 +301,7 @@ hs_lane_kernel(hs_lane_model M, hs_kernel_run P, hs_lane_state *__restrict__ sta
      * pair of each stream and stores the precomputed draws */
 #define HS_REFILL_ROUND()                                                                    \
     do {                                                                                     \
-        if (!finished && (uint32_t)(a_gen - arr_draws) + 2u <= HS_DRAW_BUF) {                \
+        if (!finished && (uint32_t)(a_gen - arr_draws) + 2u <= ARR_BUF) {                    \
             double u0_ = 0.0, u1_ = 0.0, g0_ = 1.0, g1_ = 1.0;                               \
             if (poisson && !trace_arr) { hs_uniform_pair(seed, rid, sid_arr, a_gen >> 1, &u0_, &u1_); \
                                            g0_ = hs_exp1(u0_); g1_ = hs_exp1(u1_); }         \
@@ -305,12 +312,13 @@ hs_lane_kernel(hs_lane_model M, hs_kernel_run P, hs_lane_state *__restrict__ sta
             }                                                                                \
             if (!(a_gen & 1)) {                                                              \
                 t_gen = HS_NEXT_ARRIVAL(t_gen, g0_); a_gen++;                                \
-                sh_t[a_gen % HS_DRAW_BUF][tid] = t_gen;                                      \
+                sh_t[a_gen % ARR_BUF][tid] = t_gen;                                          \
             }                                                                                \
             t_gen = HS_NEXT_ARRIVAL(t_gen, g1_); a_gen++;                                    \
-            sh_t[a_gen % HS_DRAW_BUF][tid] = t_gen;                                          \
+            sh_t[a_gen % ARR_BUF][tid] = t_gen;                                              \
         }                                                                                    \
-        if (!finished && (uint32_t)(s_gen - (uint64_t)n_svc) + 2u <= HS_DRAW_BUF) {          \
+        bool chunk_ = false;                                                                 \
+        if (!finished && (int32_t)(uint32_t)(s_gen - (uint64_t)n_svc) + 2 <= (int32_t)HS_DRAW_BUF) {   \
             double u0_ = 0.0, u1_ = 0.0;                                                     \
             int64_t d0_ = hs_seconds_to_ns(mean), d1_ = d0_;                                 \
             if (expo && !trace_svc) { hs_uniform_pair(seed, rid, sid_svc, s_gen >> 1, &u0_, &u1_); \
@@ -329,33 +337,66 @@ hs_lane_kernel(hs_lane_model M, hs_kernel_run P, hs_lane_state *__restrict__ sta
             const double s1_ = hs_ns_to_seconds(d1_);                                        \
             sh_svc[s_gen % HS_DRAW_BUF][tid] = s1_;                                          \
             s_gen++;                                                                         \
+            chunk_ = svc_chunks && (s_gen % HS_SVC_CHUNK) < 2u;   /* draws s_gen - 8 .. s_gen - 1 complete */ \
+        }                                                                                    \
+        if (FLAGS & HS_LF_REC) HS_SVC_FLUSH(chunk_);                                         \
+    } while (0)
+
+    /* The completed service chunks of the warp, written together: lane l moves draws 2 (l / 8), 2 (l / 8) + 1 of
+     * the chunk of the (l % 8)-th owner, 8 chunks per store instruction.  The chunk is the owner's whole sh_svc
+     * column, written in this round, so __syncwarp() orders those writes before the reads here (and the reads
+     * before the next round's writes).  Its ring slot follows from svc_pos = n_svc mod service_cap: the chunk
+     * starts 0..7 draws before n_svc.  Slots of draws not consumed yet are written ahead; the end of the
+     * launch puts back what they held. */
+#define HS_SVC_FLUSH(READY)                                                                  \
+    do {                                                                                     \
+        __syncwarp();                                                                        \
+        uint32_t owners_ = __ballot_sync(0xffffffffu, (READY));                              \
+        if (owners_) {                                                                       \
+            uint32_t lane_;                                                                  \
+            asm volatile("mov.u32 %0, %%laneid;" : "=r"(lane_));                             \
+            const uint32_t k_ = lane_ & 7u, pc_ = lane_ >> 3;                                \
+            const uint32_t warp_r0_ = blockIdx.x * HS_LANE_THREADS + tid - lane_;            \
+            const uint32_t back_ = (uint32_t)((uint64_t)n_svc - (s_gen - HS_SVC_CHUNK));     \
+            const uint32_t my_slot_ = svc_pos >= back_ ? svc_pos - back_ : svc_pos + P.service_cap - back_; \
+            do {                                                                             \
+                const uint32_t owner_ = min(__fns(owners_, 0u, (int)k_ + 1), 32u);           \
+                uint32_t rest_ = owners_;                                                    \
+                _Pragma("unroll") for (uint32_t q_ = 0; q_ < 8; ++q_) rest_ &= rest_ - 1u;    \
+                const uint32_t o_slot_ = __shfl_sync(0xffffffffu, my_slot_, owner_ < 32u ? owner_ : lane_); \
+                if (owner_ < 32u) {                                                          \
+                    const uint32_t col_ = tid - lane_ + owner_;                              \
+                    const uint64_t a_ = (uint64_t)__double_as_longlong(sh_svc[2u * pc_][col_]);      \
+                    const uint64_t b_ = (uint64_t)__double_as_longlong(sh_svc[2u * pc_ + 1u][col_]); \
+                    __stcs((uint4 *)(O.service + (size_t)(warp_r0_ + owner_) * P.service_cap + o_slot_) + pc_, \
+                           make_uint4((uint32_t)a_, (uint32_t)(a_ >> 32), (uint32_t)b_, (uint32_t)(b_ >> 32))); \
+                }                                                                            \
+                owners_ = rest_;                                                             \
+            } while (owners_);                                                               \
+            __syncwarp();                                                                    \
         }                                                                                    \
     } while (0)
 
-    /* Sink sample / service time into their rings, one whole 32-byte sector per global store: the first
-     * entries of a sector wait in the lane's shared-memory column, the last one completes the 256-bit
-     * store.  A sector that was begun before this launch (resume at an odd position) or rings whose
-     * capacity is not a multiple of the sector are written entry by entry. */
+    /* Sink sample into its ring: staged in the lane's shared-memory column until its 64-byte group is full,
+     * which the next loop top writes out (the fourth sample in the free record-staging row, see sh_rec).  A
+     * group that was begun before this launch (resume inside a group) or rings whose capacity is not a
+     * multiple of the group are written entry by entry. */
 #define HS_SMP_STORE(W)                                                                      \
     do {                                                                                     \
-        const uint32_t p_ = smp_pos;                                                         \
-        if (!(p_ & 1u)) smp_sync = smp_pairs;                                                \
-        if (smp_sync) { if (!(p_ & 1u)) sh_smp[tid] = (W); else hs_st256(smp + (p_ - 1u), sh_smp[tid], (W)); } \
-        else *(uint4 *)(smp + p_) = (W);                                                     \
+        const uint32_t p_ = smp_pos, q_ = p_ % HS_SMP_GROUP;                                 \
+        if (q_ == 0u) smp_sync = smp_groups;                                                 \
+        if (smp_sync) {                                                                      \
+            uint4 *d_ = (q_ < HS_SMP_GROUP - 1) ? &sh_smp[q_][tid] : &sh_rec[(st_fl + HS_STAGE - 1u) % HS_STAGE][tid]; \
+            *d_ = (W);                                                                       \
+            smp_full = (q_ == HS_SMP_GROUP - 1);                                             \
+        } else *(uint4 *)(smp + p_) = (W);                                                   \
         smp_pos = (p_ + 1 == P.sample_cap) ? 0u : p_ + 1;                                    \
     } while (0)
+    /* service time at its start: written here only when the ring does not take whole chunks */
 #define HS_SVC_STORE(V)                                                                      \
     do {                                                                                     \
-        const uint32_t p_ = svc_pos, q_ = p_ & 3u; const double v_ = (V);                    \
-        if (q_ == 0u) svc_sync = svc_quads;                                                  \
-        if (svc_sync) {                                                                      \
-            if (q_ < 3u) sh_sv[q_][tid] = v_;                                                \
-            else { const uint64_t a_ = (uint64_t)__double_as_longlong(sh_sv[0][tid]), b_ = (uint64_t)__double_as_longlong(sh_sv[1][tid]), \
-                                  c_ = (uint64_t)__double_as_longlong(sh_sv[2][tid]), d_ = (uint64_t)__double_as_longlong(v_);            \
-                   hs_st256(svc_out + (p_ - 3u), make_uint4((uint32_t)a_, (uint32_t)(a_ >> 32), (uint32_t)b_, (uint32_t)(b_ >> 32)),      \
-                            make_uint4((uint32_t)c_, (uint32_t)(c_ >> 32), (uint32_t)d_, (uint32_t)(d_ >> 32))); }                        \
-        } else svc_out[p_] = v_;                                                             \
-        svc_pos = (p_ + 1 == P.service_cap) ? 0u : p_ + 1;                                   \
+        if (!svc_chunks) svc_out[svc_pos] = (V);                                             \
+        svc_pos = (svc_pos + 1 == P.service_cap) ? 0u : svc_pos + 1;                         \
     } while (0)
 
 #define HS_RECORD(KIND, IDX, ENT)                                                            \
@@ -375,7 +416,7 @@ hs_lane_kernel(hs_lane_model M, hs_kernel_run P, hs_lane_state *__restrict__ sta
 
     /* Source.handle_event's arrival part: the next SourceEvent (source.py:166-170) */
 #define HS_NEXT_TICK()                                                                       \
-    do { arr_draws++; tT = sh_t[arr_draws % HS_DRAW_BUF][tid];                               \
+    do { arr_draws++; tT = sh_t[arr_draws % ARR_BUF][tid];                                   \
          if (tT == HS_T_EXHAUSTED) tT = INT64_MAX; else iT = ctr++; } while (0)
 
     /* Server.handle_queued_event up to its yield, for the payload (CREATED):
@@ -501,15 +542,45 @@ hs_lane_kernel(hs_lane_model M, hs_kernel_run P, hs_lane_state *__restrict__ sta
         const unsigned todo = __ballot_sync(0xffffffffu, !finished);
         if (todo == 0u) break;
         if (__any_sync(0xffffffffu, need)) HS_REFILL_ROUND();
+        /* Lanes read each other's staging here: the __syncwarp()s order the owners' earlier staging writes before
+         * these reads, and these reads before the owners' next staging writes. */
+        if (FLAGS & HS_LF_REC) __syncwarp();
+        if (FLAGS & HS_LF_REC) {
+            /* the full 64-byte Sink-sample groups of the warp, eight per store instruction: lane l moves sample l / 8
+             * of the group of the (l % 8)-th owner.  Before the record flush, which moves st_fl and with it the
+             * row that holds the fourth sample. */
+            uint32_t owners = __ballot_sync(0xffffffffu, smp_full);
+            if (owners) {
+                uint32_t lane;
+                asm volatile("mov.u32 %0, %%laneid;" : "=r"(lane));
+                const uint32_t k = lane & 7u, pc = lane >> 3;
+                const uint32_t warp_r0 = blockIdx.x * HS_LANE_THREADS + tid - lane;
+                const uint32_t my_slot = (smp_pos == 0u ? P.sample_cap : smp_pos) - HS_SMP_GROUP;
+                do {
+                    const uint32_t owner = min(__fns(owners, 0u, (int)k + 1), 32u);
+                    uint32_t rest = owners;
+#pragma unroll
+                    for (uint32_t q = 0; q < 8; ++q) rest &= rest - 1u;
+                    const uint32_t src = owner < 32u ? owner : lane;
+                    const uint32_t o_slot = __shfl_sync(0xffffffffu, my_slot, src);
+                    const uint32_t o_row = (__shfl_sync(0xffffffffu, st_fl, src) + HS_STAGE - 1u) % HS_STAGE;
+                    if (owner < 32u) {
+                        const uint32_t col = tid - lane + owner;
+                        __stcs((uint4 *)(O.samples + (size_t)(warp_r0 + owner) * P.sample_cap + o_slot + pc),
+                               pc < HS_SMP_GROUP - 1 ? sh_smp[pc][col] : sh_rec[o_row][col]);
+                    }
+                    owners = rest;
+                } while (owners);
+                __syncwarp();
+                smp_full = false;
+            }
+        }
         if ((FLAGS & HS_LF_REC) && staged) {
             /* the warp writes the full 128-byte groups of all its lanes together, four whole lines per store
              * instruction: lane l moves record l / 4 of the group of the (l % 4)-th owner of the round (so a
              * quarter-warp reads two rows of four staging columns).  An owner's group is rows 0-7 or 8-15 of
-             * its column, since st_fl is a multiple of 8; its ring slot rec_pos is group aligned.  Lanes read
-             * each other's staging here: the __syncwarp()s order the owners' earlier staging writes before
-             * these reads, and these reads before the owners' next staging writes. */
+             * its column, since st_fl is a multiple of 8; its ring slot rec_pos is group aligned. */
             const bool full = (st_wr - st_fl) >= HS_FLUSH;
-            __syncwarp();
             uint32_t owners = __ballot_sync(0xffffffffu, full);
             if (owners) {
                 /* everything below is derived from the lane index read here, so none of it is hoisted out
@@ -542,7 +613,7 @@ hs_lane_kernel(hs_lane_model M, hs_kernel_run P, hs_lane_state *__restrict__ sta
          * next arrival time, next service time, queue head */
         int64_t tT_next = 0; double sv_next = 0.0; hs_ring_entry h; h.created = 0; h.idx = 0;
         if (SIMPLE) {
-            tT_next = sh_t[(arr_draws + 1) % HS_DRAW_BUF][tid];
+            tT_next = sh_t[(arr_draws + 1) % ARR_BUF][tid];
             sv_next = sh_svc[(uint32_t)((uint64_t)n_svc % HS_DRAW_BUF)][tid];
             asm volatile("cp.async.wait_group 0;" ::: "memory");
             h = *my_head;                                    /* next queued request (meaningful if q_len > 0) */
@@ -861,15 +932,46 @@ hs_lane_kernel(hs_lane_model M, hs_kernel_run P, hs_lane_state *__restrict__ sta
     if (P.resume && S->done) return;        /* finished in an earlier window: outputs already final */
     if (FLAGS & HS_LF_BUCKETS) hs_bucket_flush(BK, r, 0u, bacc);   /* the current time bucket, at the run's end or a pause */
     if (FLAGS & HS_LF_BUCKET_PCT) status |= hs_bucket_status(BK, r);
+    if (FLAGS & HS_LF_REC) {                /* Sink samples still staged, entry by entry (before st_fl moves) */
+        if (smp_full) {
+            const uint32_t g = (smp_pos == 0u ? P.sample_cap : smp_pos) - HS_SMP_GROUP;
+            for (uint32_t q = 0; q < HS_SMP_GROUP - 1; ++q) *(uint4 *)(smp + g + q) = sh_smp[q][tid];
+            *(uint4 *)(smp + g + HS_SMP_GROUP - 1) = sh_rec[(st_fl + HS_STAGE - 1u) % HS_STAGE][tid];
+        } else if (smp_sync) {
+            for (uint32_t q = 0; q < smp_pos % HS_SMP_GROUP; ++q) *(uint4 *)(smp + smp_pos - smp_pos % HS_SMP_GROUP + q) = sh_smp[q][tid];
+        }
+    }
+    if ((FLAGS & HS_LF_REC) && svc_chunks) {
+        /* service draw j, as the refill round computes it */
+        auto service_draw = [&](uint64_t j) -> double {
+            int64_t d = hs_seconds_to_ns(mean);
+            if (expo && !trace_svc) { double u0 = 0.0, u1 = 0.0; hs_uniform_pair(seed, rid, sid_svc, j >> 1, &u0, &u1);
+                                      d = hs_exp_latency_ns_r((j & 1) ? u1 : u0, lambda, lambda_recip); }
+            if (expo && trace_svc) d = hs_seconds_to_ns(hs_div_by(trace_svc[(size_t)r * P.n_trace_svc + j], lambda, lambda_recip));
+            return hs_ns_to_seconds(d);
+        };
+        /* The refill round has written every chunk below w_end.  Draws consumed after it (w_end .. n_svc - 1, a chunk
+         * not generated whole yet) are still in the draw buffer and are written from there. */
+        const uint64_t w_end = s_gen & ~(uint64_t)(HS_SVC_CHUNK - 1);
+        uint32_t pos = svc_pos;
+        for (uint64_t j = (uint64_t)n_svc; j > w_end; --j) {
+            pos = (pos == 0u ? P.service_cap : pos) - 1u;
+            svc_out[pos] = sh_svc[(j - 1) % HS_DRAW_BUF][tid];
+        }
+        /* Undo the write-ahead: the slots of draws n_svc .. w_end - 1 were written before their service started.
+         * Each gets back what it held before this launch: the draw one ring pass earlier, or 0 if there was none (a
+         * run that is not resumed starts from zeroed rings). */
+        pos = svc_pos;
+        for (uint64_t j = (uint64_t)n_svc; j < w_end; ++j) {
+            svc_out[pos] = j >= P.service_cap ? service_draw(j - P.service_cap) : 0.0;
+            pos = (pos + 1 == P.service_cap) ? 0u : pos + 1;
+        }
+    }
     if ((FLAGS & HS_LF_REC) && staged) {    /* drain what is still staged, record by record */
         while (st_fl != st_wr) {
             __stcs((uint4 *)(rec + rec_pos), sh_rec[st_fl % HS_STAGE][tid]);
             st_fl++; rec_pos = (rec_pos + 1 == P.record_cap) ? 0u : rec_pos + 1;
         }
-    }
-    if (FLAGS & HS_LF_REC) {                /* entries of a sector that is not complete yet */
-        if (smp_sync && (smp_pos & 1u)) *(uint4 *)(smp + (smp_pos - 1u)) = sh_smp[tid];
-        if (svc_sync) for (uint32_t q = 0; q < (svc_pos & 3u); ++q) svc_out[svc_pos - (svc_pos & 3u) + q] = sh_sv[q][tid];
     }
 
     /* ---- persist / publish --------------------------------------------- */
@@ -928,6 +1030,7 @@ hs_lane_kernel(hs_lane_model M, hs_kernel_run P, hs_lane_state *__restrict__ sta
 #undef HS_SINK
 #undef HS_SMP_STORE
 #undef HS_SVC_STORE
+#undef HS_SVC_FLUSH
 #undef HS_Q_PUSH
 #undef HS_Q_POP
 #undef HS_PUSH_NOW

@@ -15,9 +15,16 @@
  *   P1b    as P1a with lane l on owner l % 4, row l / 4 (a quarter-warp reads 2 rows of 4 owners);
  *   P2     Hopper bulk copy: the owner lane issues one cp.async.bulk.global.shared::cta of its 128 B from a
  *          contiguous per-lane [lane][row] staging slice (P2w: 256 B groups of 16 records, 32 rows);
- * and, for the Sink-sample / service-time streams (data from registers, no staging):
- *   P3s    each lane writes one 32 B sector of its 2 KB ring per iteration, as two 16 B halves;
+ * and, for the Sink-sample / service-time streams (data from registers, no staging): each writer owns a 2 KB
+ * sample ring and a 1 KB service ring and fills them in the ratio of the bytes they get (a chunk of a third of
+ * the volume goes to the service ring: chunks 0, 1 of every three to the samples, chunk 2 to the service times):
+ *   P3s    each lane writes one 32 B sector per iteration, as two 16 B halves;
  *   P3w    each lane writes one 64 B chunk per iteration, as four 16 B stores;
+ *   P3q    warp-cooperative 64 B chunks: a writer has a chunk ready in about 3 of 16 iterations (the lane kernel's
+ *          rate: about one Sink sample and one service start per two loop iterations), the ready writers
+ *          (owners) are found by ballot, and each store instruction writes 8 owners' chunks, 4 lanes x 16 B each;
+ *   P3l    as P3q with whole 128 B lines, 4 owners per store instruction, 8 lanes x 16 B each (as P1b), a chunk
+ *          ready in about 3 of 32 iterations;
  *   P4     ceiling: a fully coalesced sequential write of the record volume over the same 1 GB.
  * Every pattern writes the same bytes to the same places (P0/P1/P2 record rings are checksummed against each
  * other).  GB/s = bytes written / device time (CUDA events), best and median of --reps runs, the patterns
@@ -39,8 +46,8 @@
     fprintf(stderr, "%s:%d %s: %s\n", __FILE__, __LINE__, #x, cudaGetErrorString(e_)); exit(1); } } while (0)
 
 constexpr int THREADS = 64;
-constexpr uint32_t REC_CAP = 1024, SMP_CAP = 128;  /* entries: 16 KB record and 2 KB sample rings; P3 writes the
-                                                      sample + service-time bytes into the sample rings */
+constexpr uint32_t REC_CAP = 1024, SMP_CAP = 128, SVC_CAP = 64;  /* 16 B slots: 16 KB record, 2 KB sample and 1 KB
+                                                                    service rings */
 constexpr uint32_t FULL = 0xffffffffu;
 
 __device__ __forceinline__ uint32_t mix(uint32_t x)
@@ -125,19 +132,61 @@ __global__ void __launch_bounds__(THREADS) k_records(uint4 *__restrict__ rec, co
     if (LANE_MAJOR) asm volatile("cp.async.bulk.wait_group 0;" ::: "memory");
 }
 
-/* P3s / P3w: `chunks` chunks of B bytes per writer into 2 KB sample rings, scattered, data from registers */
+/* P3s / P3w: `chunks` chunks of B bytes per writer into its 2 KB sample and 1 KB service ring, scattered, data from
+ * registers */
 template <uint32_t B>
-__global__ void __launch_bounds__(THREADS) k_sectors(uint4 *__restrict__ smp, const uint32_t *__restrict__ start_line,
-                                                     uint32_t chunks)
+__global__ void __launch_bounds__(THREADS) k_sectors(uint4 *__restrict__ smp, uint4 *__restrict__ svc,
+                                                     const uint32_t *__restrict__ start_line, uint32_t chunks)
 {
     const uint32_t w = blockIdx.x * THREADS + threadIdx.x;
-    uint4 *ring = smp + (size_t)w * SMP_CAP;
+    uint4 *const ring_s = smp + (size_t)w * SMP_CAP, *const ring_v = svc + (size_t)w * SVC_CAP;
     constexpr uint32_t E = B / 16u;
-    uint32_t pos = (start_line[w] * 8u) % SMP_CAP;
+    uint32_t pos_s = (start_line[w] * 8u) % SMP_CAP, pos_v = (start_line[w] * 8u) % SVC_CAP;
     for (uint32_t c = 0; c < chunks; ++c) {
+        const bool v = (c % 3u == 2u);
+        uint4 *const p = v ? ring_v + pos_v : ring_s + pos_s;
 #pragma unroll
-        for (uint32_t j = 0; j < E; ++j) st_cs(ring + pos + j, rec_value(w, c * E + j));
-        pos = (pos + E) % SMP_CAP;
+        for (uint32_t j = 0; j < E; ++j) st_cs(p + j, rec_value(w, c * E + j));
+        if (v) pos_v = (pos_v + E) % SVC_CAP; else pos_s = (pos_s + E) % SMP_CAP;
+    }
+}
+
+/* P3q / P3l: `chunks` chunks of B bytes per writer into the same rings, written by the warp: the owners of a round
+ * are found by ballot, lane l moves 16 B piece l / C of the chunk of the (l % C)-th owner, C = 512 / B owners per
+ * store instruction; only the owner's ring position crosses lanes */
+template <uint32_t B>
+__global__ void __launch_bounds__(THREADS) k_coop(uint4 *__restrict__ smp, uint4 *__restrict__ svc,
+                                                  const uint32_t *__restrict__ start_line, uint32_t chunks)
+{
+    constexpr uint32_t E = B / 16u, C = 32u / E;
+    const uint32_t tid = threadIdx.x, lane = tid & 31u, wbase = blockIdx.x * THREADS + (tid & ~31u);
+    const uint32_t w = blockIdx.x * THREADS + tid;
+    uint32_t pos_s = (start_line[w] * 8u) % SMP_CAP, pos_v = (start_line[w] * 8u) % SVC_CAP;
+    uint32_t c = 0;                                              /* chunks written so far */
+    const uint32_t k = lane % C, piece = lane / C;
+    for (uint32_t it = 0; __any_sync(FULL, c < chunks); ++it) {
+        const bool ready = c < chunks && (mix(w ^ (it * 0x9e3779b9u)) & 31u) < (B == 64u ? 6u : 3u);
+        const bool v = (c % 3u == 2u);
+        const uint32_t my = v ? (1u << 31) | pos_v : pos_s;     /* ring select + slot */
+        uint32_t owners = __ballot_sync(FULL, ready);
+        while (owners) {
+            const uint32_t owner = min(__fns(owners, 0u, (int)k + 1), 32u);
+            uint32_t rest = owners;
+#pragma unroll
+            for (uint32_t q = 0; q < C; ++q) rest &= rest - 1u;
+            const uint32_t src = owner < 32u ? owner : lane;
+            const uint32_t o_my = __shfl_sync(FULL, my, src), o_c = __shfl_sync(FULL, c, src);
+            if (owner < 32u) {
+                const uint32_t ow = wbase + owner;
+                uint4 *base = (o_my >> 31) ? svc + (size_t)ow * SVC_CAP : smp + (size_t)ow * SMP_CAP;
+                st_cs(base + (o_my & 0x7fffffffu) + piece, rec_value(ow, o_c * E + piece));
+            }
+            owners = rest;
+        }
+        if (ready) {
+            if (v) pos_v = (pos_v + E) % SVC_CAP; else pos_s = (pos_s + E) % SMP_CAP;
+            c++;
+        }
     }
 }
 
@@ -180,14 +229,15 @@ int main(int argc, char **argv)
     CK(cudaGetDeviceProperties(&prop, 0));
     printf("# device: %s, %d SMs, %.0f MHz max SM clock, L2 %d MB\n", prop.name, prop.multiProcessorCount,
            prop.clockRate / 1e3, prop.l2CacheSize >> 20);
-    printf("# %u writers x (16 KB + 2 KB) rings, seeded random start lines (seed %u); %.3g events: %u record groups "
+    printf("# %u writers x (16 KB + 2 KB + 1 KB) rings, seeded random start lines (seed %u); %.3g events: %u record groups "
            "and %u sample/service sectors per writer\n", W, seed, events, groups, sectors);
 
-    uint4 *rec = nullptr, *smp = nullptr;
+    uint4 *rec = nullptr, *smp = nullptr, *svc = nullptr;
     uint32_t *start = nullptr;
     unsigned long long *sum = nullptr;
     CK(cudaMalloc(&rec, (size_t)W * REC_CAP * 16));
     CK(cudaMalloc(&smp, (size_t)W * SMP_CAP * 16));
+    CK(cudaMalloc(&svc, (size_t)W * SVC_CAP * 16));
     CK(cudaMalloc(&start, W * 4));
     CK(cudaMalloc(&sum, 8));
     std::vector<uint32_t> h(W);
@@ -205,6 +255,8 @@ int main(int argc, char **argv)
         {"P2w", "owner lane, cp.async.bulk 256 B from [lane][row] staging (+17 KB smem)", (double)W * (groups / 2) * 256.0, true},
         {"P3s", "scattered 32 B sectors, two 16 B halves (sample/service pattern)", sec_bytes, false},
         {"P3w", "scattered 64 B chunks, four 16 B stores", (double)W * (sectors / 2) * 64.0, false},
+        {"P3q", "warp-cooperative 64 B chunks, 8 chunks per store, 4 lanes x 16 B each", (double)W * (sectors / 2) * 64.0, false},
+        {"P3l", "warp-cooperative 128 B lines, 4 lines per store, 8 lanes x 16 B each", (double)W * (sectors / 4) * 128.0, false},
         {"P4", "fully coalesced sequential write (ceiling)", rec_bytes, false},
     };
     auto launch = [&](int p) {
@@ -214,9 +266,11 @@ int main(int argc, char **argv)
         case 2: k_records<P1B><<<blocks, THREADS>>>(rec, start, groups); break;
         case 3: k_records<P2><<<blocks, THREADS>>>(rec, start, groups); break;
         case 4: k_records<P2W><<<blocks, THREADS>>>(rec, start, groups / 2); break;
-        case 5: k_sectors<32><<<blocks, THREADS>>>(smp, start, sectors); break;
-        case 6: k_sectors<64><<<blocks, THREADS>>>(smp, start, sectors / 2); break;
-        case 7: k_sequential<<<blocks, THREADS>>>(rec, (size_t)W * REC_CAP - 1, (size_t)W * groups * 8); break;
+        case 5: k_sectors<32><<<blocks, THREADS>>>(smp, svc, start, sectors); break;
+        case 6: k_sectors<64><<<blocks, THREADS>>>(smp, svc, start, sectors / 2); break;
+        case 7: k_coop<64><<<blocks, THREADS>>>(smp, svc, start, sectors / 2); break;
+        case 8: k_coop<128><<<blocks, THREADS>>>(smp, svc, start, sectors / 4); break;
+        case 9: k_sequential<<<blocks, THREADS>>>(rec, (size_t)W * REC_CAP - 1, (size_t)W * groups * 8); break;
         }
         CK(cudaGetLastError());
     };
@@ -258,6 +312,6 @@ int main(int argc, char **argv)
     bool same = true;
     for (int p = 1; p < 4; ++p) same &= sums[p] == sums[0];
     printf("# record rings identical across P0/P1a/P1b/P2: %s\n", same ? "yes" : "NO");
-    CK(cudaFree(rec)); CK(cudaFree(smp)); CK(cudaFree(start)); CK(cudaFree(sum));
+    CK(cudaFree(rec)); CK(cudaFree(smp)); CK(cudaFree(svc)); CK(cudaFree(start)); CK(cudaFree(sum));
     return same ? 0 : 1;
 }
