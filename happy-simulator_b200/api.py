@@ -1132,17 +1132,28 @@ class ParallelRunner:
         return _ReplicaResults(sim, out, _time.monotonic() - t0)
 
     def run_sweep(self, configs: list[RunConfig]) -> list[ParallelResult]:
+        """Configurations of one topology run as the cells of one launch.  A ``build_fn`` may also return a
+        ParallelSimulation: linked ones of one linked topology run as the cells of one linked ensemble
+        (``parallel._run_linked_sweep``), and each result's ``summary`` is that configuration's
+        ParallelSimulationSummary.  Results keep the order of ``configs``."""
+        from .parallel import ParallelSimulation, _run_linked_sweep
         if not configs:
             return []
-        sims = []
+        built = []
         for cfg in configs:
             sim = cfg.build_fn()
             if cfg.seed is not None:
                 sim._seed = int(cfg.seed)
-            sims.append(sim)
+            built.append(sim)
+        res: list = [None] * len(built)
+        par = [i for i, sm in enumerate(built) if isinstance(sm, ParallelSimulation)]
+        if par:
+            for i, (summ, status) in zip(par, _run_linked_sweep([built[i] for i in par])):
+                res[i] = ParallelResult(name=configs[i].name, summary=summ, status=status)
+        idx = [i for i, sm in enumerate(built) if not isinstance(sm, ParallelSimulation)]
+        sims = [built[i] for i in idx]
         for sm in sims:                 # cancellations are part of the topology: read them before grouping
             lowering.refresh_fault_cancellation(sm.model)
-        res: list = [None] * len(sims)
         for g in _group_by_topology(sims):
             seeds = [sims[i]._seed for i in g]
             rids = [sims[i]._replica for i in g]
@@ -1154,5 +1165,5 @@ class ParallelRunner:
             else:            # seeds that are not an arithmetic progression: one launch each
                 sums = [sims[i].run() for i in g]
             for i, sm in zip(g, sums):
-                res[i] = ParallelResult(name=configs[i].name, summary=sm, status=sims[i].last_run_info.get("status", 0))
+                res[idx[i]] = ParallelResult(name=configs[idx[i]].name, summary=sm, status=sims[i].last_run_info.get("status", 0))
         return res

@@ -14,6 +14,7 @@
 #include <cstring>
 #include <algorithm>
 #include <array>
+#include <map>
 #include <string>
 #include <utility>
 #include <vector>
@@ -1209,19 +1210,29 @@ int hs_totals_device_ptr(hs_engine *E, void **ptr)
 #define HS_MAX_LINKS_ 16
 struct hs_link_dev { int32_t kind, stream; double mean_s, loss; hs_xevent *inbox; uint32_t *inbox_n; uint32_t inbox_cap, pad; };
 struct hs_links_dev { hs_link_dev l[HS_MAX_LINKS_]; };
+struct hs_link_cell { double mean_s, loss; };           /* the per-cell columns of one link */
+
+/* a source engine's per-cell link table on the device, [n_cells][n_links]; `host` is what was last uploaded */
+struct hs_cell_links { std::vector<hs_link_cell> host; dev_buf dev; };
 
 struct hs_coordinator {
     int device = 0; cudaStream_t stream = nullptr;
     uint32_t n = 0, n_streams = 1;
     uint64_t seed = 0, seed_stride = 0; uint32_t rid_base = 0, rid_stride = 0, index_base = 0;
     dev_buf d_loss_draws, d_lat_draws, d_counts;      /* uint64[n], uint64[n][n_streams], uint64[3][n] */
+    std::map<const hs_engine *, hs_cell_links> cell_links;      /* hs_coordinator_exchange_cells, per source engine */
 };
 
 /* one thread per replica: its outbox in emission order -- one loss draw when the link loses packets, then
- * event.time = send_time + latency.sample(), then Simulation.schedule(event) = a slot of the destination's inbox */
+ * event.time = send_time + latency.sample(), then Simulation.schedule(event) = a slot of the destination's inbox.
+ * CELLS: the latency mean and the loss come from the replica's sweep cell, row (g / replicas_per_cell) % n_cells of
+ * cells[n_cells][n_links]; kind, latency object and destination are the link's in every cell. */
+} /* extern "C" */
+template <bool CELLS>
 __global__ void hs_exchange_kernel(const hs_xevent *__restrict__ outbox, uint32_t *__restrict__ outbox_n, uint32_t ocap,
                                    const hs_entity_desc *__restrict__ src_ents, hs_links_dev LK, uint32_t n, uint32_t n_streams,
                                    uint64_t seed0, uint64_t seed_stride, uint32_t rid_base, uint32_t rid_stride, uint32_t index_base,
+                                   const hs_link_cell *__restrict__ cells, uint32_t n_links, uint32_t replicas_per_cell, uint32_t n_cells,
                                    uint64_t *__restrict__ loss_draws, uint64_t *__restrict__ lat_draws, uint64_t *__restrict__ counts)
 {
     const uint32_t r = blockIdx.x * blockDim.x + threadIdx.x;
@@ -1230,17 +1241,20 @@ __global__ void hs_exchange_kernel(const hs_xevent *__restrict__ outbox, uint32_
     const uint64_t seed = seed0 + (uint64_t)g * seed_stride;
     const uint32_t rid = rid_base + g * rid_stride;
     const uint32_t cnt = outbox_n[r];
+    const hs_link_cell *cl = CELLS ? cells + (size_t)((g / replicas_per_cell) % n_cells) * n_links : nullptr;
     uint64_t nl = loss_draws[r], delivered = 0, lost = 0, over = 0;
     for (uint32_t k = 0; k < cnt; ++k) {
         const hs_xevent x = outbox[(size_t)r * ocap + k];
         const hs_entity_desc row = src_ents[x.ent];
         const hs_link_dev &L = LK.l[row.i0];
-        if (L.loss > 0.0 && hs_uniform(seed, rid, HS_STREAM_LINK_LOSS, nl++) < L.loss) { lost++; continue; }
+        double loss = L.loss, mean_s = L.mean_s;
+        if (CELLS) { const hs_link_cell c = cl[row.i0]; loss = c.loss; mean_s = c.mean_s; }
+        if (loss > 0.0 && hs_uniform(seed, rid, HS_STREAM_LINK_LOSS, nl++) < loss) { lost++; continue; }
         int64_t lat;
         if (L.kind == HS_SVC_EXPONENTIAL) {
             const uint64_t d = lat_draws[(size_t)r * n_streams + L.stream]++;
-            lat = hs_exp_latency_ns(hs_uniform(seed, rid, HS_STREAM_LINK_LATENCY | ((uint32_t)L.stream << 8), d), HS_DIV(1.0, L.mean_s));
-        } else lat = hs_seconds_to_ns(L.mean_s);
+            lat = hs_exp_latency_ns(hs_uniform(seed, rid, HS_STREAM_LINK_LATENCY | ((uint32_t)L.stream << 8), d), HS_DIV(1.0, mean_s));
+        } else lat = hs_seconds_to_ns(mean_s);
         const uint32_t m = L.inbox_n[r];
         if (m >= L.inbox_cap) { over++; continue; }
         hs_xevent y = x; y.time_ns = x.time_ns + lat; y.ent = row.i1;
@@ -1252,6 +1266,7 @@ __global__ void hs_exchange_kernel(const hs_xevent *__restrict__ outbox, uint32_
     loss_draws[r] = nl;
     counts[r] += delivered; counts[(size_t)n + r] += lost; counts[2 * (size_t)n + r] += over;
 }
+extern "C" {
 
 int hs_coordinator_create(int device, void *cuda_stream, uint32_t n_replicas, uint32_t n_streams,
                           uint64_t seed, uint64_t seed_stride, uint32_t rid_base, uint32_t rid_stride,
@@ -1281,13 +1296,35 @@ void hs_coordinator_destroy(hs_coordinator *c)
     if (!c) return;
     cudaSetDevice(c->device);
     c->d_loss_draws.release(); c->d_lat_draws.release(); c->d_counts.release();
+    for (auto &t : c->cell_links) t.second.dev.release();
     delete c;
 }
 
-int hs_coordinator_exchange(hs_coordinator *c, hs_engine *src, uint32_t n_links, const hs_link_desc *links, hs_engine *const *dsts)
+int hs_link_cells_validate(uint32_t n_links, uint32_t n_cells, const hs_link_desc *links)
+{
+    if (!n_cells || n_links > HS_MAX_LINKS_ || (n_links && !links)) return fail(HS_ERR_INVALID, "hs_link_cells_validate: bad arguments (at most %d links, n_cells >= 1)", HS_MAX_LINKS_);
+    for (uint32_t cell = 0; cell < n_cells; ++cell)
+        for (uint32_t k = 0; k < n_links; ++k) {
+            const hs_link_desc &a = links[k], &b = links[(size_t)cell * n_links + k];
+            if (b.latency_kind != HS_SVC_CONSTANT && b.latency_kind != HS_SVC_EXPONENTIAL) return fail(HS_ERR_INVALID, "link %u, cell %u: bad latency kind", k, cell);
+            if (b.latency_kind != a.latency_kind) return fail(HS_ERR_INVALID, "link %u: latency kind differs between cell 0 and cell %u", k, cell);
+            if (b.stream != a.stream) return fail(HS_ERR_INVALID, "link %u: latency stream differs between cell 0 and cell %u", k, cell);
+            if (!(b.latency_mean_s >= 0.0) || !(b.packet_loss >= 0.0 && b.packet_loss < 1.0))
+                return fail(HS_ERR_INVALID, "link %u, cell %u: latency must be >= 0 and packet_loss in [0, 1) (parallel/link.py:45-52)", k, cell);
+        }
+    return HS_OK;
+}
+
+/* hs_coordinator_exchange (n_cells = 0) and hs_coordinator_exchange_cells (links = [n_cells][n_links]) */
+static int exchange(hs_coordinator *c, hs_engine *src, uint32_t n_links, uint32_t n_cells, uint32_t replicas_per_cell,
+                    const hs_link_desc *links, hs_engine *const *dsts)
 {
     if (!c || !src) return fail(HS_ERR_INVALID, "hs_coordinator_exchange: NULL handle");
     if (n_links > HS_MAX_LINKS_ || (n_links && (!links || !dsts))) return fail(HS_ERR_INVALID, "hs_coordinator_exchange: at most %d links", HS_MAX_LINKS_);
+    if (n_cells) {       /* a malformed table is refused whether or not the partition ran */
+        const int rc = hs_link_cells_validate(n_links, n_cells, links);
+        if (rc) return rc;
+    }
     if (!src->have_run || !src->outbox_cap) return HS_OK;              /* nothing can have been sent */
     if (src->link_replicas != c->n) return fail(HS_ERR_STATE, "the coordinator was created for %u replicas, the partition ran %u", c->n, src->link_replicas);
     CUDA_TRY(cudaSetDevice(c->device));
@@ -1315,14 +1352,44 @@ int hs_coordinator_exchange(hs_coordinator *c, hs_engine *src, uint32_t n_links,
         if (D->stream != c->stream) { foreign = true; CUDA_TRY(cudaStreamSynchronize(D->stream)); }
     }
     if (src->stream != c->stream) CUDA_TRY(cudaStreamSynchronize(src->stream));
+    const hs_link_cell *d_cells = nullptr;
+    if (n_cells) {
+        /* uploaded once per run: every window passes the same table, so only the first barrier (or a changed table)
+         * copies it; the copy is ordered on the coordinator's stream behind the kernels that read the old one */
+        std::vector<hs_link_cell> tab((size_t)n_cells * n_links);
+        for (size_t i = 0; i < tab.size(); ++i) tab[i] = hs_link_cell{links[i].latency_mean_s, links[i].packet_loss};
+        hs_cell_links &T = c->cell_links[src];
+        if (T.host.size() != tab.size() || (tab.size() && memcmp(T.host.data(), tab.data(), tab.size() * sizeof(hs_link_cell)))) {
+            int rc;
+            if ((rc = T.dev.ensure(std::max<size_t>(1, tab.size()) * sizeof(hs_link_cell)))) return rc;
+            T.host = std::move(tab);
+            if (!T.host.empty())
+                CUDA_TRY(cudaMemcpyAsync(T.dev.p, T.host.data(), T.host.size() * sizeof(hs_link_cell), cudaMemcpyHostToDevice, c->stream));
+        }
+        d_cells = (const hs_link_cell *)T.dev.p;
+    }
     const uint32_t threads = 128, blocks = (c->n + threads - 1) / threads;
-    hs_exchange_kernel<<<blocks, threads, 0, c->stream>>>((const hs_xevent *)src->d_outbox.p, (uint32_t *)src->d_outbox_n.p, src->outbox_cap,
+    auto kernel = n_cells ? hs_exchange_kernel<true> : hs_exchange_kernel<false>;
+    kernel<<<blocks, threads, 0, c->stream>>>((const hs_xevent *)src->d_outbox.p, (uint32_t *)src->d_outbox_n.p, src->outbox_cap,
         (const hs_entity_desc *)src->d_ents.p, LK, c->n, c->n_streams, c->seed, c->seed_stride, c->rid_base, c->rid_stride, c->index_base,
+        d_cells, n_links, replicas_per_cell, n_cells,
         (uint64_t *)c->d_loss_draws.p, (uint64_t *)c->d_lat_draws.p, (uint64_t *)c->d_counts.p);
     CUDA_TRY(cudaGetLastError());
     if (foreign) CUDA_TRY(cudaStreamSynchronize(c->stream));      /* a partition on another stream must not run ahead of the barrier */
     src->launches += 1;
     return HS_OK;
+}
+
+int hs_coordinator_exchange(hs_coordinator *c, hs_engine *src, uint32_t n_links, const hs_link_desc *links, hs_engine *const *dsts)
+{
+    return exchange(c, src, n_links, 0, 1, links, dsts);
+}
+
+int hs_coordinator_exchange_cells(hs_coordinator *c, hs_engine *src, uint32_t n_links, uint32_t n_cells, uint32_t replicas_per_cell,
+                                  const hs_link_desc *links, hs_engine *const *dsts)
+{
+    if (!n_cells || !replicas_per_cell) return fail(HS_ERR_INVALID, "hs_coordinator_exchange_cells: n_cells and replicas_per_cell must be >= 1");
+    return exchange(c, src, n_links, n_cells, replicas_per_cell, links, dsts);
 }
 
 int hs_coordinator_read(hs_coordinator *c, uint64_t *delivered, uint64_t *lost, uint64_t *overflowed)

@@ -29,7 +29,8 @@ EXPORTED_SYMBOLS = ["hs_version", "hs_last_error", "hs_engine_create", "hs_engin
                     "hs_model_validate", "hs_run", "hs_set_trace", "hs_sync", "hs_last_run_ms", "hs_launch_count",
                     "hs_last_launch", "hs_read_outputs", "hs_read_totals", "hs_read_cell_totals", "hs_totals_device_ptr",
                     "hs_sketch_layout", "hs_read_sketches", "hs_coordinator_create", "hs_coordinator_destroy",
-                    "hs_coordinator_exchange", "hs_coordinator_read", "hs_read_outbox", "hs_read_inbox",
+                    "hs_coordinator_exchange", "hs_coordinator_exchange_cells", "hs_link_cells_validate",
+                    "hs_coordinator_read", "hs_read_outbox", "hs_read_inbox",
                     "hs_partition_upload", "hs_partition_validate", "hs_set_buckets", "hs_read_buckets",
                     "hs_read_bucket_totals", "hs_set_bucket_percentiles", "hs_read_bucket_percentiles",
                     "hs_read_bucket_percentile_totals"]
@@ -76,6 +77,8 @@ def load_library(path: str | None = None):
                                    C.c_uint32, C.POINTER(H)], C.c_int),
         "hs_coordinator_destroy": ([H], None),
         "hs_coordinator_exchange": ([H, H, C.c_uint32, C.POINTER(A.LinkDesc), C.POINTER(H)], C.c_int),
+        "hs_coordinator_exchange_cells": ([H, H, C.c_uint32, C.c_uint32, C.c_uint32, C.POINTER(A.LinkDesc), C.POINTER(H)], C.c_int),
+        "hs_link_cells_validate": ([C.c_uint32, C.c_uint32, C.POINTER(A.LinkDesc)], C.c_int),
         "hs_coordinator_read": ([H, C.POINTER(C.c_uint64), C.POINTER(C.c_uint64), C.POINTER(C.c_uint64)], C.c_int),
         "hs_read_outbox": ([H, C.c_void_p, C.POINTER(C.c_uint32)], C.c_int),
         "hs_read_inbox": ([H, C.c_void_p, C.POINTER(C.c_uint32)], C.c_int),
@@ -124,6 +127,13 @@ def make_params(*, seed=1234, end_ns, n_replicas=1, seed_stride=0, rid_base=0, r
     return p
 
 
+def validate_link_cells(links, n_links: int, n_cells: int) -> None:
+    """hs_link_cells_validate: the checks hs_coordinator_exchange_cells makes of a per-cell link table (ctypes
+    hs_link_desc array of n_cells * n_links), without a device."""
+    L = load_library()
+    _check(L, L.hs_link_cells_validate(n_links, n_cells, links))
+
+
 class Coordinator:
     """The window barrier of a linked run (hs_coordinator_*, parallel/coordinator.py:182-227): per-replica draw
     counters of the loss stream and the links' latency streams, delivery totals."""
@@ -136,11 +146,16 @@ class Coordinator:
         _check(self._L, self._L.hs_coordinator_create(device, C.c_void_p(stream or 0), n_replicas, n_streams, seed, seed_stride, rid_base,
                                                       rid_stride, replica_index_base, C.byref(self._h)))
 
-    def exchange(self, src: "Engine", links, dsts) -> None:
+    def exchange(self, src: "Engine", links, dsts, n_cells: int = 0, replicas_per_cell: int = 1) -> None:
         """Drain ``src``'s outboxes through its outgoing ``links`` (ctypes hs_link_desc array) into the inboxes of the
-        engines ``dsts`` (one per link slot)."""
+        engines ``dsts`` (one per link slot).  With ``n_cells`` > 0, ``links`` is the per-cell table [n_cells][slot]
+        and replica g sends through row (g / replicas_per_cell) % n_cells (hs_coordinator_exchange_cells)."""
         arr = (C.c_void_p * max(1, len(dsts)))(*[d._h for d in dsts])
-        _check(self._L, self._L.hs_coordinator_exchange(self._h, src._h, len(dsts), links, arr))
+        if n_cells:
+            _check(self._L, self._L.hs_coordinator_exchange_cells(self._h, src._h, len(dsts), n_cells, replicas_per_cell,
+                                                                   links, arr))
+        else:
+            _check(self._L, self._L.hs_coordinator_exchange(self._h, src._h, len(dsts), links, arr))
 
     def read(self):
         """(delivered, lost, overflowed) uint64[n_replicas] since creation."""

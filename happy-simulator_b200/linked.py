@@ -10,7 +10,10 @@ float arithmetic of coordinator.py:88-95, and every partition runs window after 
 ``hs_run(end_ns=window end, resume=window > 0)``; ``hs_coordinator_exchange`` moves the outboxes at each barrier."""
 from __future__ import annotations
 
+import dataclasses
 from dataclasses import dataclass, field
+
+import numpy as np
 
 from . import _abi as A
 from .model import FlatModel
@@ -34,10 +37,49 @@ class LinkedModel:
     window_s: float
     n_streams: int = 1
     objects: list[list] = field(default_factory=list)     # per partition: entity id -> user object (lowering)
+    # sweep cells: per partition float64 [n_cells, slot, 2], every link's (latency_mean_s, packet_loss) in every cell;
+    # the partitions' models carry the cells' rows (FlatModel.cell_d0 / cell_i0).  None: one configuration, ``links``.
+    cell_links: list[np.ndarray] | None = None
 
     @property
     def n_partitions(self) -> int:
         return len(self.models)
+
+    @property
+    def n_cells(self) -> int:
+        """Sweep cells of the run (0: none).  Replica g runs cell (g / replicas_per_cell) % n_cells everywhere."""
+        return 0 if self.cell_links is None else int(self.cell_links[0].shape[0])
+
+    @classmethod
+    def from_cells(cls, cells: list["LinkedModel"]) -> "LinkedModel":
+        """One LinkedModel whose cell c is ``cells[c]``: models, links and windows of one linked topology (the caller
+        checks that), differing at most in the models' d0 / server i0 and the links' latency mean and loss."""
+        lead = cells[0]
+        models = []
+        for q, m in enumerate(lead.models):
+            mm = dataclasses.replace(m, cell_d0=np.stack([np.asarray(c.models[q].entities["d0"], np.float64) for c in cells]),
+                                     cell_i0=np.stack([np.asarray(c.models[q].entities["i0"], np.int32) for c in cells]))
+            mm.outbox_cap = max(int(c.models[q].outbox_cap) for c in cells)
+            mm.inbox_cap = max(int(c.models[q].inbox_cap) for c in cells)
+            models.append(mm)
+        tab = [np.array([[(float(l.latency_mean_s), float(l.packet_loss)) for l in c.links[q]] for c in cells],
+                        np.float64).reshape(len(cells), len(lead.links[q]), 2) for q in range(lead.n_partitions)]
+        return cls(models, list(lead.names), [list(ls) for ls in lead.links], window_s=lead.window_s,
+                   n_streams=lead.n_streams, objects=lead.objects, cell_links=tab)
+
+    def cell(self, c: int) -> "LinkedModel":
+        """The plain LinkedModel (no cells) of cell ``c``: its rows written into the models, its link parameters."""
+        if not self.n_cells:
+            return self
+        models = []
+        for m in self.models:
+            E = m.entities.copy()
+            E["d0"], E["i0"] = m.cell_d0[c], m.cell_i0[c]
+            models.append(dataclasses.replace(m, entities=E, cell_d0=None, cell_i0=None))
+        links = [[dataclasses.replace(l, latency_mean_s=float(t[c, k, 0]), packet_loss=float(t[c, k, 1]))
+                  for k, l in enumerate(ls)] for ls, t in zip(self.links, self.cell_links)]
+        return LinkedModel(models, list(self.names), links, window_s=self.window_s, n_streams=self.n_streams,
+                           objects=self.objects)
 
     def window_ends(self, end_ns: int, start_ns: int = 0) -> list[int]:
         """WindowedCoordinator.run's window ends (coordinator.py:86-96): float seconds, clamped to the end time,
@@ -59,12 +101,20 @@ class LinkedModel:
         return ends
 
     def link_descs(self, p: int):
-        """(ctypes hs_link_desc array, destination partition indices) of partition p's outgoing links."""
-        arr = (A.LinkDesc * max(1, len(self.links[p])))()
-        for k, l in enumerate(self.links[p]):
-            arr[k].latency_kind, arr[k].stream = int(l.latency_kind), int(l.stream)
-            arr[k].latency_mean_s, arr[k].packet_loss = float(l.latency_mean_s), float(l.packet_loss)
-        return arr, [int(l.dest) for l in self.links[p]]
+        """(ctypes hs_link_desc array, destination partition indices) of partition p's outgoing links.  With cells the
+        array is the per-cell table [n_cells][slot] of hs_coordinator_exchange_cells."""
+        ls = self.links[p]
+        nc = max(1, self.n_cells)
+        arr = (A.LinkDesc * max(1, nc * len(ls)))()
+        for c in range(nc):
+            for k, l in enumerate(ls):
+                d = arr[c * len(ls) + k]
+                d.latency_kind, d.stream = int(l.latency_kind), int(l.stream)
+                if self.n_cells:
+                    d.latency_mean_s, d.packet_loss = (float(v) for v in self.cell_links[p][c, k])
+                else:
+                    d.latency_mean_s, d.packet_loss = float(l.latency_mean_s), float(l.packet_loss)
+        return arr, [int(l.dest) for l in ls]
 
     def validate(self) -> None:
         for p, ls in enumerate(self.links):
@@ -86,6 +136,14 @@ class LinkedModel:
                                      f"{self.names[self.links[p][slot].dest]!r}, which cannot receive requests")
             if m.ids_of(A.HS_ENT_REMOTE) and m.outbox_cap <= 0:
                 raise ValueError(f"partition {self.names[p]!r} has REMOTE rows but no outbox")
+        if self.cell_links is not None:
+            nc = self.n_cells
+            for p, (m, t) in enumerate(zip(self.models, self.cell_links)):
+                if t.shape != (nc, len(self.links[p]), 2) or m.n_cells != nc:
+                    raise ValueError(f"partition {self.names[p]!r}: {m.n_cells} model cells and a link table of shape "
+                                     f"{t.shape}, the run has {nc} cells of {len(self.links[p])} links")
+                if not ((t[..., 0] >= 0).all() and (t[..., 1] >= 0).all() and (t[..., 1] < 1).all()):
+                    raise ValueError(f"partition {self.names[p]!r}: a cell's link latency is < 0 or its loss outside [0, 1)")
 
 
 class LinkedRun:
@@ -119,9 +177,14 @@ class LinkedRun:
             self.coordinator.close()
 
     def run(self, *, seed, end_ns, n_replicas=1, replica_index_base=0, caps=None, flags=A.HS_RUN_ORDER_HASH, queue_ring=0,
-            buckets=None, bucket_sample_cap=0):
+            buckets=None, bucket_sample_cap=0, replicas_per_cell=1, seed_stride=0, rid_stride=None):
         """caps: per-partition dicts of record_cap / sample_cap / service_cap (or one dict for all).  Returns the
         per-partition outputs (Engine.read_outputs) and (delivered, lost, overflowed) per replica.
+
+        Replica g draws with Philox key ``seed + g * seed_stride``; partition q with replica word ``q + g * rid_stride``,
+        the coordinator with ``P + g * rid_stride`` (rid_stride defaults to P + 1).  With cells (``LinkedModel.n_cells``)
+        replica g runs cell (g / replicas_per_cell) % n_cells in every partition and at every barrier, and every
+        partition's outputs get ``cell_totals`` (Engine.read_cell_totals).
 
         ``buckets=(width_s, n)`` (checked by the caller, with no recorder rings in ``caps``) buckets the samples of
         every partition that has a Sink, tracker or Probe row; ``bucket_sample_cap`` > 0 adds their p50 / p99.  Those
@@ -129,10 +192,13 @@ class LinkedRun:
         from . import buckets as _buckets
         from . import engine as _engine
         lm, nP = self.lm, self.lm.n_partitions
+        nc = lm.n_cells
+        rs = nP + 1 if rid_stride is None else int(rid_stride)
         if self.coordinator is not None:
             self.coordinator.close()
-        self.coordinator = _engine.Coordinator(self.device, n_replicas, lm.n_streams, seed=seed, rid_base=nP,
-                                               rid_stride=nP + 1, replica_index_base=replica_index_base, stream=self._stream_ptr)
+        self.coordinator = _engine.Coordinator(self.device, n_replicas, lm.n_streams, seed=seed, seed_stride=seed_stride,
+                                               rid_base=nP, rid_stride=rs, replica_index_base=replica_index_base,
+                                               stream=self._stream_ptr)
         caps = caps or {}
         link_args = [lm.link_descs(q) for q in range(nP)]
         ends = lm.window_ends(end_ns)
@@ -144,18 +210,23 @@ class LinkedRun:
             for w, wend in enumerate(ends):
                 for q, e in enumerate(self.engines):
                     c = caps[q] if isinstance(caps, (list, tuple)) else caps
-                    e.run(_engine.make_params(seed=seed, end_ns=wend, n_replicas=n_replicas, rid_base=q, rid_stride=nP + 1,
-                                              replica_index_base=replica_index_base, engine=3, resume=1 if w else 0,
+                    e.run(_engine.make_params(seed=seed, seed_stride=seed_stride, end_ns=wend, n_replicas=n_replicas,
+                                              rid_base=q, rid_stride=rs, replica_index_base=replica_index_base,
+                                              replicas_per_cell=replicas_per_cell, engine=3, resume=1 if w else 0,
                                               flags=flags | A.HS_RUN_LINKED, queue_ring=queue_ring, **c))
                 for q, e in enumerate(self.engines):
                     arr, dst = link_args[q]
                     if dst:
-                        self.coordinator.exchange(e, arr, [self.engines[d] for d in dst])
+                        self.coordinator.exchange(e, arr, [self.engines[d] for d in dst], nc, replicas_per_cell)
             self.windows = len(ends)
             outs = [e.read_outputs() for e in self.engines]
+            if nc:
+                for o, e in zip(outs, self.engines):
+                    o["cell_totals"] = e.read_cell_totals(nc)
             for q in bucketed:
                 objs = lm.objects[q] if lm.objects else [None] * lm.models[q].n_entities
-                outs[q].update(_buckets.read_outputs(self.engines[q], buckets, bucket_sample_cap, lm.models[q], objs))
+                outs[q].update(_buckets.read_outputs(self.engines[q], buckets, bucket_sample_cap, lm.models[q], objs,
+                                                     max(1, nc)))
         finally:
             for e in self.engines:          # the engines may run again without buckets
                 e.set_bucket_percentiles(0)

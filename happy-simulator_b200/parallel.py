@@ -73,8 +73,11 @@ class ParallelSimulationSummary:
 
 def _reaching_rates(lm) -> list[float]:
     """Per partition of a LinkedModel: the summed peak rate of every source whose requests can reach it -- its own
-    and those of every partition upstream of it over links, followed transitively."""
+    and those of every partition upstream of it over links, followed transitively.  With sweep cells: the largest
+    over the cells, each with its own rates."""
     from .lowering import source_rate_bound
+    if lm.n_cells:
+        return [max(v) for v in zip(*(_reaching_rates(lm.cell(c)) for c in range(lm.n_cells)))]
     own = [source_rate_bound(m) for m in lm.models]
     upstream: list[set[int]] = [set() for _ in lm.models]
     for p, ls in enumerate(lm.links):
@@ -116,6 +119,89 @@ def _short_rings(outs, caps) -> list[tuple[int, str, int]]:
             if (cap != "record_cap" or c[cap]) and n > c[cap]:
                 short.append((q, cap, n))
     return short
+
+
+def _linked_difference(a, b) -> str | None:
+    """What keeps two linked ParallelSimulations from running as the cells of one linked ensemble, or None when they
+    can: the same partitions in the same order, partition models of one topology (``api._same_topology``), the same
+    links (source, destination, latency kind, which links share a latency object), the same windows and end time, the
+    same ``link_buffer`` and device.  Latency means, packet losses, rates, mean service times and concurrency may
+    differ: they are the per-cell columns."""
+    from .api import _same_topology
+    la, lb = a._linked, b._linked
+    if la is None or lb is None:
+        return "a ParallelSimulation without PartitionLinks"
+    if la.names != lb.names:
+        return f"partitions {la.names} and {lb.names}"
+    for q, name in enumerate(la.names):
+        if not _same_topology(la.models[q], lb.models[q]):
+            return f"partition {name!r}: the models differ in more than rates, mean service times and concurrency"
+        x, y = la.links[q], lb.links[q]
+        if [(l.dest, l.latency_kind, l.stream) for l in x] != [(l.dest, l.latency_kind, l.stream) for l in y]:
+            return f"partition {name!r}: links differ in destination, latency kind or shared latency objects"
+    if la.n_streams != lb.n_streams:
+        return "links differ in shared latency objects"
+    if la.window_s != lb.window_s:
+        return f"window {la.window_s} s and {lb.window_s} s"
+    if a._end_ns != b._end_ns:
+        return f"end time {a._end_ns} ns and {b._end_ns} ns"
+    if a.link_buffer != b.link_buffer:
+        return f"link_buffer {a.link_buffer} and {b.link_buffer}"
+    if a._device != b._device:
+        return f"device {a._device} and {b._device}"
+    return None
+
+
+def _same_linked_topology(a, b) -> bool:
+    """Two linked ParallelSimulations that can run as cells of one linked ensemble (``_linked_difference``)."""
+    return _linked_difference(a, b) is None
+
+
+def _replica_status(outs, r: int) -> int:
+    st = 0
+    for o in outs:
+        st |= int(o["summaries"]["status"][r])
+    return st
+
+
+def _run_linked_sweep(sims) -> list:
+    """ParallelRunner.run_sweep's ParallelSimulations: (ParallelSimulationSummary, status) per configuration, in order.
+    Linked configurations of one topology (``_same_linked_topology``) whose seeds form an arithmetic progression run as
+    ONE linked ensemble, configuration k as replica k of cell k with Philox key ``seed_0 + k * (seed_1 - seed_0)`` and
+    the replica words of a single run (rid_stride 0), so that each equals its own ``run()``; results are written back
+    onto each configuration's own objects.  The others, and ParallelSimulations without links, run one by one."""
+    from .linked import LinkedModel
+    from .lowering import refresh_fault_cancellation
+    res: list = [None] * len(sims)
+    groups: list[list[int]] = []
+    for i, sm in enumerate(sims):
+        if sm._linked is None:
+            res[i] = (sm.run(), 0)
+            continue
+        for m in sm._linked.models:     # cancellations are part of the topology: read them before grouping
+            refresh_fault_cancellation(m)
+        for g in groups:
+            if _same_linked_topology(sims[g[0]], sm):
+                g.append(i)
+                break
+        else:
+            groups.append([i])
+    for g in groups:
+        seeds = [int(sims[i]._seed) for i in g]
+        ds = {b - a for a, b in zip(seeds, seeds[1:])}
+        if len(g) > 1 and len(ds) <= 1 and min(ds | {0}) >= 0:
+            lead = sims[g[0]]
+            lm = LinkedModel.from_cells([sims[i]._linked for i in g])
+            ring = max(int(getattr(sims[i], "queue_ring", 0) or 0) for i in g)
+            outs, delivered, lost, wall, windows = lead._run_linked(
+                len(g), 0, lm=lm, seed=seeds[0], seed_stride=ds.pop() if ds else 0, rid_stride=0, queue_ring=ring)
+            for k, i in enumerate(g):
+                res[i] = (sims[i]._summarise_linked(outs, delivered, lost, wall, windows, replica=k), _replica_status(outs, k))
+        else:            # seeds that are not an arithmetic progression: one run each
+            for i in g:
+                summ = sims[i].run()
+                res[i] = (summ, _replica_status(sims[i].last_outputs, 0))
+    return res
 
 
 def _aggregate(summaries: dict[str, SimulationSummary]) -> dict:
@@ -252,15 +338,29 @@ class ParallelSimulation:
     link_buffer = 256        # cross-partition events one replica may emit per window (class default; overflow is reported)
     queue_ring = 0           # device slots per server queue of a linked run (0: the engine's default); grown and re-run on overflow
 
-    def _run_linked(self, n_replicas: int = 1, replica_index_base: int = 0, buckets=None, bucket_sample_cap: int = 0):
+    def _run_linked(self, n_replicas: int = 1, replica_index_base: int = 0, buckets=None, bucket_sample_cap: int = 0, *,
+                    lm=None, seed=None, seed_stride: int = 0, rid_stride=None, replicas_per_cell: int = 1, queue_ring=None):
+        """The linked run of ``self._linked``, or of ``lm`` (a LinkedModel with sweep cells, of this one's topology):
+        ring sizing, growth and re-runs.  ``seed`` (default: this simulation's), ``seed_stride``, ``rid_stride`` and
+        ``replicas_per_cell`` are LinkedRun.run's."""
         from . import _abi as A
         from . import buckets as _buckets
         from .api import EnsembleStatusError, Instant
         from .linked import LinkedRun
         from .lowering import refresh_fault_cancellation
-        lm = self._linked
-        for m in lm.models:                 # FaultHandle.cancel() may have been called since the partitions were lowered
-            refresh_fault_cancellation(m)
+        if lm is None:
+            lm = self._linked
+            for m in lm.models:             # FaultHandle.cancel() may have been called since the partitions were lowered
+                refresh_fault_cancellation(m)
+        seed = self._seed if seed is None else seed
+        # a run without cells or strides calls LinkedRun.run exactly as before these existed
+        stride_kw = {}
+        if lm.n_cells:
+            stride_kw["replicas_per_cell"] = replicas_per_cell
+        if seed_stride:
+            stride_kw["seed_stride"] = seed_stride
+        if rid_stride is not None:
+            stride_kw["rid_stride"] = rid_stride
         t0 = _time.monotonic()
         run = LinkedRun(lm, device=self._device)
         cap = bucket_sample_cap
@@ -281,7 +381,7 @@ class ParallelSimulation:
             # `caps` are always what the last attempt ran with.
             # With percentiles, a time bucket that outgrew the sample capacity is no failure either: the whole run is
             # repeated once with the capacity that holds every bucket (as Simulation.run_ensemble's "grow").
-            ring = int(getattr(self, "queue_ring", 0) or 0)
+            ring = int((getattr(self, "queue_ring", 0) if queue_ring is None else queue_ring) or 0)
             ok = _TIES | (A.HS_ST_BUCKET_OVERFLOW if cap else 0)
             queue_full, short, cap_short, cap_grown = False, [], False, False
             for attempt in range(6):
@@ -293,9 +393,9 @@ class ParallelSimulation:
                     cap = max(_buckets.sample_cap_needed(o["buckets"]) for o in outs if "buckets" in o)
                     cap_grown = True
                 bk = dict(buckets=buckets, bucket_sample_cap=cap) if buckets is not None else {}
-                outs, (delivered, lost, over) = run.run(seed=self._seed, end_ns=self._end_ns, n_replicas=n_replicas,
+                outs, (delivered, lost, over) = run.run(seed=seed, end_ns=self._end_ns, n_replicas=n_replicas,
                                                         replica_index_base=replica_index_base, caps=caps, flags=0, queue_ring=ring,
-                                                        **bk)
+                                                        **bk, **stride_kw)
                 status = 0
                 for o in outs:
                     status |= int(np.bitwise_or.reduce(o["summaries"]["status"])) if len(o["summaries"]) else 0
@@ -347,40 +447,75 @@ class ParallelSimulation:
             return self._summarise_linked(*self._run_linked(1))
         return self._run_independent()
 
-    def _summarise_linked(self, outs, delivered, lost, wall, windows) -> ParallelSimulationSummary:
+    def _summarise_linked(self, outs, delivered, lost, wall, windows, replica: int = 0) -> ParallelSimulationSummary:
         """coordinator.py:123-172: per-partition summaries from the partitions' final state, the aggregate like
-        _build_summary; results are written back onto the script's own objects (replica 0)."""
-        lm = self._linked
+        _build_summary; results are written back onto the script's own objects (replica ``replica`` of ``outs``)."""
+        lm, r = self._linked, replica
         summaries = {}
         for q, name in enumerate(lm.names):
-            write_back(lm.models[q], lm.objects[q], outs[q], 0, Instant)
+            write_back(lm.models[q], lm.objects[q], outs[q], r, Instant)
             entities = [o for o in self._partitions[q].entities if any(o is x for x in lm.objects[q])]
-            summaries[name] = replica_summary(outs[q]["summaries"][0], wall, entities,
-                                              events_cancelled=fault_cancelled(lm.models[q], outs[q]["entity_stats"][0]))
+            summaries[name] = replica_summary(outs[q]["summaries"][r], wall, entities,
+                                              events_cancelled=fault_cancelled(lm.models[q], outs[q]["entity_stats"][r]))
         n = len(summaries)
         return ParallelSimulationSummary(
             **_aggregate(summaries), wall_clock_seconds=wall,
             partition_wall_times={nm: wall / n for nm in summaries}, speedup=1.0, parallelism_efficiency=1.0 / n if n else 1.0,
-            total_windows=windows, total_cross_partition_events=int(delivered[0]), window_size_s=lm.window_s)
+            total_windows=windows, total_cross_partition_events=int(delivered[r]), window_size_s=lm.window_s)
 
-    def run_ensemble(self, n_replicas: int, replica_index_base: int = 0, *, buckets=None, bucket_percentiles: bool = False,
-                     bucket_sample_cap: int = 64):
+    def run_ensemble(self, n_replicas: int, replica_index_base: int = 0, *, cells=None, replicas_per_cell: int = 1,
+                     buckets=None, bucket_percentiles: bool = False, bucket_sample_cap: int = 64):
         """Linked partitions only: n replicas of the whole ParallelSimulation in one set of launches.  Returns
         {partition name: per-replica outputs (Engine.read_outputs)}, delivered and lost cross-partition events per
         replica.
 
+        ``cells``: linked ParallelSimulations of this one's linked topology (``_same_linked_topology``: they may differ
+        in rates, mean service times, concurrency, link latency means and packet losses) and seed, run as the sweep
+        cells of this ensemble: replica g runs cell (g / replicas_per_cell) % len(cells), the configuration
+        ``cells[cell]``, and draws exactly as replica g of ``cells[cell].run_ensemble(n)``.  Every partition's outputs
+        then hold ``cell_totals`` (Engine.read_cell_totals), and bucket totals are per cell.
+
         ``buckets=(width_s, n)``, ``bucket_percentiles`` and ``bucket_sample_cap`` are those of
         ``Simulation.run_ensemble``: every partition with a Sink, tracker or Probe gets its time buckets (and p50 / p99)
-        under the same keys (one cell), and ``buckets.bucketed_data(outs[name], obj, replica)`` reads them.  Such a run
+        under the same keys, and ``buckets.bucketed_data(outs[name], obj, replica)`` reads them.  Such a run
         keeps no recorder rings, so its memory does not grow with the horizon.  A bucket with more than
         ``bucket_sample_cap`` samples makes the run repeat once with the capacity that holds them all."""
         from . import buckets as _buckets
         if self._linked is None:
             raise UnsupportedModelError("run_ensemble is for partitions joined by PartitionLinks")
+        if int(replicas_per_cell) < 1:
+            raise ValueError("replicas_per_cell must be >= 1")
         spec = _buckets.check_spec(buckets, self._end_ns) if buckets is not None else None
         cap = _buckets.check_sample_cap(bucket_sample_cap, spec) if bucket_percentiles else 0
-        outs, delivered, lost, wall, windows = self._run_linked(n_replicas, replica_index_base, spec, cap)   # a rank's shard: base = rank * n
+        kw = {}
+        if cells is not None:
+            kw = dict(lm=self._cells_model(cells), replicas_per_cell=int(replicas_per_cell),
+                      queue_ring=max(int(getattr(c, "queue_ring", 0) or 0) for c in [self, *cells]))
+        outs, delivered, lost, wall, windows = self._run_linked(n_replicas, replica_index_base, spec, cap, **kw)   # a rank's shard: base = rank * n
         return {n: o for n, o in zip(self._linked.names, outs)}, delivered, lost
+
+    def _cells_model(self, cells):
+        """The LinkedModel whose cell c is ``cells[c]``; refuses cells of another linked topology or seed."""
+        from .linked import LinkedModel
+        from .lowering import refresh_fault_cancellation
+        cells = list(cells)
+        if not cells:
+            raise ValueError("cells must hold at least one ParallelSimulation")
+        for k, c in enumerate(cells):
+            if not isinstance(c, ParallelSimulation) or c._linked is None:
+                raise UnsupportedModelError(f"cells[{k}] is not a ParallelSimulation with PartitionLinks")
+            for m in c._linked.models:
+                refresh_fault_cancellation(m)
+        for m in self._linked.models:
+            refresh_fault_cancellation(m)
+        for k, c in enumerate(cells):
+            why = _linked_difference(self, c)
+            if why is not None:
+                raise UnsupportedModelError(f"cells[{k}] is not of this ParallelSimulation's linked topology: {why}")
+            if int(c._seed) != int(self._seed):
+                raise UnsupportedModelError(f"cells[{k}] has seed {c._seed}, this ParallelSimulation {self._seed}: the "
+                                            "cells of one ensemble share its seed")
+        return LinkedModel.from_cells([c._linked for c in cells])
 
     def _run_independent(self) -> ParallelSimulationSummary:
         """Independent partitions (parallel/simulation.py:170-195).  Partitions whose lowered models share a

@@ -507,6 +507,19 @@ void hs_coordinator_destroy(hs_coordinator *c);
  * engine pushes its inbox into the replicas' heaps before the first pop (Simulation.schedule, :195-206). */
 int hs_coordinator_exchange(hs_coordinator *c, hs_engine *src, uint32_t n_links, const hs_link_desc *links,
                             hs_engine *const *dsts);
+/* hs_coordinator_exchange for a linked run whose replicas are sweep cells: links[cell][k], n_cells rows of n_links, and
+ * replica g (= replica_index_base + r) sends through row (g / replicas_per_cell) % n_cells -- the cell the partitions'
+ * hs_model_desc.cell_d0 / cell_i0 give it.  latency_mean_s and packet_loss may differ between the rows; latency_kind
+ * and stream (which latency object a link draws from) must be equal in every row, and the destination dsts[k] is one
+ * for all cells.  Each replica draws exactly as hs_coordinator_exchange with its row's values: a loss draw only when
+ * its cell's packet_loss is > 0.  The table is kept on the device per source engine and copied again only when its
+ * bytes change, so the windows of a run upload it once.  hs_coordinator_exchange is the one-cell case of the same
+ * barrier. */
+int hs_coordinator_exchange_cells(hs_coordinator *c, hs_engine *src, uint32_t n_links, uint32_t n_cells,
+                                  uint32_t replicas_per_cell, const hs_link_desc *links, hs_engine *const *dsts);
+/* The checks hs_coordinator_exchange_cells makes of links[n_cells][n_links], without a device: a valid latency kind,
+ * latency_mean_s >= 0 and packet_loss in [0, 1) in every row, latency_kind and stream equal to row 0's. */
+int hs_link_cells_validate(uint32_t n_links, uint32_t n_cells, const hs_link_desc *links);
 /* per-replica totals since create ([n_replicas] each, any pointer may be NULL): events delivered into inboxes,
  * events lost on lossy links, events that found the destination's inbox full (a sizing error: raise inbox_cap) */
 int hs_coordinator_read(hs_coordinator *c, uint64_t *delivered, uint64_t *lost, uint64_t *overflowed);

@@ -4,6 +4,7 @@ lossy fan-out, many replicas, timed with a host clock around LinkedRun.run endin
 
     python tools/bench_linked.py [--faults] [replicas ...]
     python tools/bench_linked.py --buckets W N [--percentiles] [--long] [replicas ...]
+    python tools/bench_linked.py --sweep K [--rpc R] [--sim-s S]
 
 --faults runs every configuration a second time with a node-fault schedule in every partition (fault_schedules):
 the same ensemble then runs the LINKED | FAULTS kernels, and the two lines compare their throughput.
@@ -15,6 +16,12 @@ card and its power limit, read in the same process.  N must cover every configur
 N > 100 / W).  --long adds the point a record-mode run could not hold: tandem_heavy
 (500 req/s) for 100 s at 16 384 replicas, with buckets only (its recorder rings would need about 5 MB per
 partition-replica, 165 GB in all).
+
+--sweep K runs K configurations of linked_tandem_const (link latency 1x to 1.875x the window, mean service times 0.6x
+to 1.4x), R replicas each (default 1), for S simulated seconds (default 20) in two ways, alternating, 5 rounds each: K
+separate LinkedRuns, and one LinkedRun whose K sweep cells are the configurations (LinkedModel.from_cells, K * R
+replicas).  Each is timed with a host clock that ends in a device synchronise, outputs read included; the line gives
+both medians, whether every configuration's summaries came out the same both ways, and the card and its power limit.
 """
 import json
 import math
@@ -141,10 +148,86 @@ def bench_buckets(args):
         print(json.dumps(line), flush=True)
 
 
+def sweep_configs(lm, K):
+    """K LinkedModels of lm's topology: server mean service times 0.6x to 1.4x, link latency 1x to 1.875x"""
+    import dataclasses
+    out = []
+    for k in range(K):
+        models = []
+        for m in lm.models:
+            E = m.entities.copy()
+            srv = E["kind"] == A.HS_ENT_SERVER
+            E["d0"][srv] = E["d0"][srv] * (0.6 + 0.8 * k / max(1, K - 1))
+            models.append(dataclasses.replace(m, entities=E))
+        links = [[dataclasses.replace(l, latency_mean_s=l.latency_mean_s * (1 + (k % 8) / 8)) for l in ls] for ls in lm.links]
+        out.append(dataclasses.replace(lm, models=models, links=links))
+    return out
+
+
+def bench_sweep(args):
+    """--sweep K [--rpc R] [--sim-s S]: K separate LinkedRuns against one celled LinkedRun, alternating, median of 5"""
+    from happysim_b200.linked import LinkedModel
+    opt = lambda f, d: type(d)(args[args.index(f) + 1]) if f in args else d      # noqa: E731
+    K, rpc, end_s = opt("--sweep", 16), opt("--rpc", 1), opt("--sim-s", 20.0)
+    name_, limit = card()
+    lm, kw, z = G.load_linked("linked_tandem_const")
+    cfgs = sweep_configs(lm, K)
+    celled = LinkedModel.from_cells(cfgs)
+    end_ns, seed = int(end_s * 1e9), kw["seed"]
+
+    def separate():
+        res = []
+        for k, c in enumerate(cfgs):       # configuration k's replicas keep their global index, hence their draws
+            run = LinkedRun(c)
+            try:
+                outs, counts = run.run(seed=seed, end_ns=end_ns, n_replicas=rpc, replica_index_base=k * rpc, flags=0)
+            finally:
+                run.close()
+            res.append(outs)
+        return res
+
+    def one():
+        run = LinkedRun(celled)
+        try:
+            return run.run(seed=seed, end_ns=end_ns, n_replicas=K * rpc, replicas_per_cell=rpc, flags=0)
+        finally:
+            run.close()
+
+    def clock(fn):
+        torch.cuda.synchronize()
+        t0 = time.perf_counter()
+        r = fn()
+        torch.cuda.synchronize()
+        return time.perf_counter() - t0, r
+
+    separate(), one()                # warm-up (module load, allocations)
+    t_sep, t_one = [], []
+    for _ in range(5):
+        dt, sep = clock(separate)
+        t_sep.append(dt)
+        dt, (outs, counts) = clock(one)
+        t_one.append(dt)
+    same = all(outs[q]["summaries"][k * rpc:(k + 1) * rpc].tobytes() == sep[k][q]["summaries"].tobytes()
+               for k in range(K) for q in range(lm.n_partitions))
+    bits = 0
+    for o in outs:
+        bits |= int(np.bitwise_or.reduce(o["summaries"]["status"]))
+    ev = sum(int(o["summaries"]["events_processed"].sum()) for o in outs)
+    a, b = statistics.median(t_sep), statistics.median(t_one)
+    print(json.dumps({"mode": "sweep", "model": "linked_tandem_const", "configs": K, "replicas_per_config": rpc,
+                      "sim_s": end_s, "windows": len(lm.window_ends(end_ns)), "events": ev, "status_bits": bits,
+                      "separate_runs_ms": round(a * 1e3, 2), "celled_run_ms": round(b * 1e3, 2),
+                      "speedup": round(a / b, 2), "same_summaries": same, "rounds": 5,
+                      "timed": "host clock around the runs (outputs read), ending in a device synchronise",
+                      "card": name_, "power_limit": limit}), flush=True)
+
+
 def main():
     args = sys.argv[1:]
     if "--buckets" in args:
         return bench_buckets(args)
+    if "--sweep" in args:
+        return bench_sweep(args)
     faults = "--faults" in args
     sizes = [int(a) for a in args if a != "--faults"] or [4096, 16384, 65536]
     for (name, end_s), with_faults in [(c, f) for c in (("linked_tandem_const", 20.0), ("linked_lossy_fanout", 10.0))
