@@ -155,6 +155,18 @@ __device__ __forceinline__ int64_t hs_lane_next_arrival(int64_t t, double target
     return n < t ? INT64_MAX : n;
 }
 
+/* lane of the k-th lowest set bit of mask (k < K; 32: fewer than k + 1 bits set), the owner a lane serves in a round of
+ * the recorder's warp-wide flushes.  The same result as min(__fns(mask, 0, k + 1), 32), in K - 1 predicated steps and
+ * one find-first: __fns is a branchy binary search of about 50 dependent instructions, run once per round of every
+ * flush, where it made up most of the flush's latency. */
+template <uint32_t K>
+__device__ __forceinline__ uint32_t hs_kth_set_lane(uint32_t mask, uint32_t k)
+{
+#pragma unroll
+    for (uint32_t q = 0; q + 1 < K; ++q) mask = q < k ? mask & (mask - 1u) : mask;
+    return mask ? (uint32_t)(__ffs((int)mask) - 1) : 32u;
+}
+
 template <int FLAGS>
 __global__ void __launch_bounds__(HS_LANE_THREADS, 7)
 hs_lane_kernel(hs_lane_model M, hs_kernel_run P, hs_lane_state *__restrict__ states,
@@ -360,7 +372,7 @@ hs_lane_kernel(hs_lane_model M, hs_kernel_run P, hs_lane_state *__restrict__ sta
             const uint32_t back_ = (uint32_t)((uint64_t)n_svc - (s_gen - HS_SVC_CHUNK));     \
             const uint32_t my_slot_ = svc_pos >= back_ ? svc_pos - back_ : svc_pos + P.service_cap - back_; \
             do {                                                                             \
-                const uint32_t owner_ = min(__fns(owners_, 0u, (int)k_ + 1), 32u);           \
+                const uint32_t owner_ = hs_kth_set_lane<8>(owners_, k_);                     \
                 uint32_t rest_ = owners_;                                                    \
                 _Pragma("unroll") for (uint32_t q_ = 0; q_ < 8; ++q_) rest_ &= rest_ - 1u;    \
                 const uint32_t o_slot_ = __shfl_sync(0xffffffffu, my_slot_, owner_ < 32u ? owner_ : lane_); \
@@ -557,7 +569,7 @@ hs_lane_kernel(hs_lane_model M, hs_kernel_run P, hs_lane_state *__restrict__ sta
                 const uint32_t warp_r0 = blockIdx.x * HS_LANE_THREADS + tid - lane;
                 const uint32_t my_slot = (smp_pos == 0u ? P.sample_cap : smp_pos) - HS_SMP_GROUP;
                 do {
-                    const uint32_t owner = min(__fns(owners, 0u, (int)k + 1), 32u);
+                    const uint32_t owner = hs_kth_set_lane<8>(owners, k);
                     uint32_t rest = owners;
 #pragma unroll
                     for (uint32_t q = 0; q < 8; ++q) rest &= rest - 1u;
@@ -591,9 +603,8 @@ hs_lane_kernel(hs_lane_model M, hs_kernel_run P, hs_lane_state *__restrict__ sta
                 const uint32_t k = lane & 3u, row = lane >> 2;
                 const uint32_t warp_r0 = blockIdx.x * HS_LANE_THREADS + tid - lane;   /* replica of lane 0 */
                 do {
-                    /* the k-th lowest owner left (32: none); __fns instead of a search loop keeps <10> free of
-                     * spills */
-                    const uint32_t owner = min(__fns(owners, 0u, (int)k + 1), 32u);
+                    /* the k-th lowest owner left (32: none) */
+                    const uint32_t owner = hs_kth_set_lane<4>(owners, k);
                     uint32_t rest = owners;
 #pragma unroll
                     for (uint32_t q = 0; q < 4; ++q) rest &= rest - 1u;
