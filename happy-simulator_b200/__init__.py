@@ -19,7 +19,8 @@ from .sketching import (HyperLogLog, CountMinSketch, BloomFilter, TopK, Reservoi
                         KeyExtractor, FrequencyEstimate, TDigest, QuantileEstimator, LatencyExtractor)  # noqa: F401,E402
 from .api import (  # noqa: F401,E402
     Instant, Duration, Entity, Source, SimpleEventProvider, ConstantRateProfile, ConstantArrivalTimeProvider,
-    PoissonArrivalTimeProvider, ConstantLatency, ExponentialLatency, FIFOQueue, LIFOQueue, FixedConcurrency,
+    PoissonArrivalTimeProvider, ConstantLatency, ExponentialLatency, FIFOQueue, LIFOQueue, PriorityQueue, PriorityByKey,
+    FixedConcurrency,
     Server, ServerStats, CachingServer, CachingServerStats, Sink, Counter, LoadBalancer, LoadBalancerStats, RoundRobin, ConsistentHash,
     UniformKeyContext, ZipfKeyContext, StepProfile, Simulation, SimulationSummary, EntitySummary, QueueStats, ParallelRunner, RunConfig,
     ParallelResult, seed, run_lowered, LinearRampProfile, SpikeProfile,

@@ -16,7 +16,7 @@ METRICS = {"depth": 0, "active_requests": 1, "utilization": 2, "available_capaci
            "stats_dropped": 5, "events_received": 6, "total": 7, "generated_count": 8}
 HS_ARR_CONSTANT, HS_ARR_POISSON = 0, 1
 HS_SVC_CONSTANT, HS_SVC_EXPONENTIAL = 0, 1
-HS_Q_FIFO, HS_Q_LIFO = 0, 1
+HS_Q_FIFO, HS_Q_LIFO, HS_Q_PRIORITY = 0, 1, 2
 HS_LB_ROUND_ROBIN, HS_LB_KEY_TABLE = 0, 1
 HS_PROF_CONSTANT, HS_PROF_LINEAR_RAMP, HS_PROF_SPIKE, HS_PROF_STEP = 0, 1, 2, 3
 

@@ -245,6 +245,32 @@ class LIFOQueue(FIFOQueue):
     """components/queue_policy.py:117-156"""
 
 
+class PriorityQueue(FIFOQueue):
+    """components/queue_policy.py:189-287: pops the request with the smallest (key(request), insertion order).  On the
+    device the key is a ``PriorityByKey`` table over the request's routing key; ``_insert_counter`` (successful pushes)
+    is published after a run, as the reference's object would hold it."""
+
+    def __init__(self, capacity: float = float("inf"), key: Callable | None = None):
+        super().__init__(capacity)
+        self._key = key
+        self._insert_counter = 0
+
+
+class PriorityByKey:
+    """key for PriorityQueue: the priority of a request is ``values[k]``, k its routing key
+    (``context["metadata"]["client_id"]`` of ``UniformKeyContext`` / ``ZipfKeyContext``), the one per-request value
+    that exists on the device.  Lower values leave first.  A plain callable, so the same object works as the key of
+    the reference's own PriorityQueue."""
+
+    priority_by_routing_key = True
+
+    def __init__(self, values):
+        self.values = list(values)
+
+    def __call__(self, event):
+        return self.values[event.context["metadata"]["client_id"]]
+
+
 class FixedConcurrency:
     """components/server/concurrency.py:66-140"""
 

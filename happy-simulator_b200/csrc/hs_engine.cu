@@ -176,7 +176,22 @@ static int validate_model(const hs_model_desc *m, bool partition = false)
             if (e.target >= (int32_t)n) return fail(HS_ERR_INVALID, "entity %u: downstream out of range", i);
             if (e.target >= 0 && m->entities[e.target].kind == HS_ENT_SOURCE) return fail(HS_ERR_INVALID, "entity %u: downstream is a source", i);
             if (e.i0 < 1) return fail(HS_ERR_INVALID, "entity %u: max_concurrent must be >= 1, got %d (concurrency.py:86)", i, e.i0);
-            if (e.i1 != HS_Q_FIFO && e.i1 != HS_Q_LIFO) return fail(HS_ERR_INVALID, "entity %u: bad queue policy", i);
+            if (e.i1 != HS_Q_FIFO && e.i1 != HS_Q_LIFO && e.i1 != HS_Q_PRIORITY) return fail(HS_ERR_INVALID, "entity %u: bad queue policy", i);
+            if (e.i1 != HS_Q_PRIORITY && e.i3 != 0) return fail(HS_ERR_INVALID, "entity %u: i3 of a FIFO / LIFO server is reserved (0)", i);
+            if (e.i1 == HS_Q_PRIORITY) {    /* PriorityQueue: one priority per routing key, in profile_table at i3 - 1 */
+                int32_t pop = 0;
+                for (uint32_t j = 0; j < n; ++j) {
+                    const hs_entity_desc &s_ = m->entities[j];
+                    if (s_.kind != HS_ENT_SOURCE) continue;
+                    if (s_.i1 <= 0 && (s_.target < 0 || (uint32_t)s_.target >= n || m->entities[s_.target].kind != HS_ENT_PROBE))
+                        return fail(HS_ERR_INVALID, "entity %u: a PriorityQueue server needs a routing key on every request (source %u draws none)", i, j);
+                    pop = std::max(pop, s_.i1);
+                }
+                if (e.i3 < 1 || !m->profile_table || (uint64_t)(e.i3 - 1) + (uint64_t)pop > m->n_profile_table)
+                    return fail(HS_ERR_INVALID, "entity %u: priority table out of range (it must cover %d keys)", i, pop);
+                for (int32_t k = 0; k < pop; ++k)
+                    if (m->profile_table[(e.i3 - 1) + k] != m->profile_table[(e.i3 - 1) + k]) return fail(HS_ERR_INVALID, "entity %u: priority of key %d is NaN", i, k);
+            }
             if (e.i2 != HS_SVC_CONSTANT && e.i2 != HS_SVC_EXPONENTIAL) return fail(HS_ERR_INVALID, "entity %u: bad service kind", i);
             if (e.i2 == HS_SVC_EXPONENTIAL && !(e.d0 > 0.0)) return fail(HS_ERR_INVALID, "entity %u: exponential mean must be > 0", i);
             if (e.d0 < 0.0) return fail(HS_ERR_INVALID, "entity %u: negative service time", i);
@@ -324,6 +339,7 @@ static bool classify_lane(hs_engine *E)
         else return false;
     }
     if (src < 0 || srv < 0) return false;
+    if (en[srv].i1 == HS_Q_PRIORITY) return false;        /* the lane kernel keeps a FIFO / LIFO ring only */
     if (en[src].target != srv || en[src].i1 != 0) return false;
     if (en[srv].target != dst) { if (!(en[srv].target < 0 && dst < 0)) return false; }
     const int32_t c_max = max_concurrency(E, (uint32_t)srv);
@@ -471,6 +487,7 @@ static int general_setup(hs_engine *E, const hs_kernel_run &R, bool thread, bool
     M.profiles = (const hs_profile_desc *)E->d_profiles.p;
     M.sketch_tables = (const int32_t *)E->d_sketch_tab.p; M.sk_total = E->sk_total;
     M.key_cdf = (const double *)E->d_key_cdf.p;
+    M.profile_table = (const double *)E->d_profile_table.p;
     M.n_entities = ne; M.n_cells = E->n_cells; M.n_servers = n_servers; M.fel_slots = S; M.block_bytes = block_bytes;
     M.n_backends = (uint32_t)E->backends.size(); M.model_bytes = 0;
     M.outbox_cap = E->outbox_cap; M.inbox_cap = E->inbox_cap;
@@ -813,6 +830,8 @@ int hs_run(hs_engine *E, const hs_run_params *p)
     if (faults && linked && !E->partition)
         return fail(HS_ERR_INVALID, "a linked partition with FAULT rows (a fault schedule) is uploaded with hs_partition_upload");
     if (engine == 2 && faults) return fail(HS_ERR_INVALID, "the lane engine does not run fault schedules (the model has FAULT rows): use engine 0, 1 or 3");
+    if (engine == 2 && std::any_of(E->ents.begin(), E->ents.end(), [](const hs_entity_desc &e) { return e.kind == HS_ENT_SERVER && e.i1 == HS_Q_PRIORITY; }))
+        return fail(HS_ERR_INVALID, "the lane engine does not run PriorityQueue servers (queue policy HS_Q_PRIORITY): use engine 0, 1 or 3");
     if (engine == 2 && !E->lane_ok) return fail(HS_ERR_INVALID, "lane engine needs Source -> Server(concurrency <= 64) -> Sink|Counter");
 
     if (E->bkt_cap && !E->bkt_n)

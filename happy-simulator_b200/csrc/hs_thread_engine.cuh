@@ -510,7 +510,8 @@ hs_thread_body(const hs_warp_model &M, const hs_kernel_run &P, unsigned char *__
                 const uint32_t srv_idx = (uint32_t)__double_as_longlong(dv.d1) & 0xffffffu;
                 hs_wring_entry *rg = ring0 + (size_t)srv_idx * P.ring;
                 hs_wring_entry q; q.created = now; q.idx = idxE; q.key = key;
-                rg[(q_head + q_len) & ring_mask] = q;
+                if (dv.i1 == HS_Q_PRIORITY) hs_pq_push(rg, q_len, q, (uint32_t)(Xv->u.srv.accepted - 1), M.profile_table + (dv.i3 - 1));
+                else rg[(q_head + q_len) & ring_mask] = q;
                 Xv->u.srv.q_len = q_len + 1;
             }
             went_store((int)ent, xs);
@@ -535,7 +536,8 @@ hs_thread_body(const hs_warp_model &M, const hs_kernel_run &P, unsigned char *__
             double svc_s = 0.0; int64_t resume_t = 0;
             hs_wring_entry q; q.created = 0; q.idx = 0; q.key = -1;
             if (start) {
-                /* the waiting request first: its load (a miss, as a rule) is in flight while the service time is drawn */
+                /* the waiting request first: its load (a miss, as a rule) is in flight while the service time is drawn.
+                 * A PriorityQueue's root is slot 0 = q_head: the same load; the heap is repaired below */
                 const uint32_t srv_idx = (uint32_t)__double_as_longlong(dv.d1) & 0xffffffu;
                 const hs_wring_entry *rg = ring0 + (size_t)srv_idx * P.ring;
                 q = rg[(dv.i1 == HS_Q_LIFO ? q_head + q_len - 1 : q_head) & ring_mask];
@@ -581,7 +583,9 @@ hs_thread_body(const hs_warp_model &M, const hs_kernel_run &P, unsigned char *__
                     emit(now, idxD, HS_EV_DELIVER, ent);
                     emit(now, q.idx, HS_EV_REQ_WORKER, ent);
                     ctr++;                                             /* inline ProcessContinuation */
-                    Xv->u.srv.q_head = (q_len == 1) ? 0u : (dv.i1 != HS_Q_LIFO ? q_head + 1 : q_head);   /* empty: restart at slot 0 */
+                    if (dv.i1 == HS_Q_PRIORITY)
+                        hs_pq_pop(ring0 + (size_t)((uint32_t)__double_as_longlong(dv.d1) & 0xffffffu) * P.ring, q_len, M.profile_table + (dv.i3 - 1));
+                    else Xv->u.srv.q_head = (q_len == 1) ? 0u : (dv.i1 != HS_Q_LIFO ? q_head + 1 : q_head);   /* empty: restart at slot 0 */
                     Xv->u.srv.q_len = q_len - 1;
                     act = active + 1;
                     if (dv.i2 == HS_SVC_EXPONENTIAL) Xv->u.srv.svc_draws = svc_draws + 1;

@@ -86,6 +86,60 @@ struct __align__(16) hs_went {          /* 96 B per entity */
 
 struct hs_wring_entry { int64_t created; uint64_t idx; int64_t key; };   /* 24 B */
 
+/* PriorityQueue (components/queue_policy.py:189-287) of an HS_Q_PRIORITY server: a binary min-heap in slots
+ * 0 .. q_len - 1 of the server's queue ring (q_head stays 0), ordered by (tab[routing key], insertion sequence) --
+ * the reference's (priority, insert_order), a total order, so any heap pops what its heapq pops.  The sequence is the
+ * server's accepted count at push time (PriorityQueue._insert_counter counts successful pushes), kept as 32 bits in
+ * the upper half of the entry's key; compared modulo 2^32, it orders the entries exactly as long as the oldest and
+ * the newest waiting request are fewer than 2^31 accepted requests apart.  The entry's idx (the payload's sort
+ * index) is not the insertion order: a request delivered over a link carries the sending partition's index. */
+__device__ __forceinline__ bool hs_pq_less(const double pa, const uint32_t sa, const double pb, const uint32_t sb)
+{
+    return pa < pb || (pa == pb && (int32_t)(sa - sb) < 0);
+}
+__device__ __forceinline__ double hs_pq_prio(const hs_wring_entry &e, const double *tab) { return tab[(int32_t)e.key]; }
+__device__ __forceinline__ uint32_t hs_pq_seq(const hs_wring_entry &e) { return (uint32_t)((uint64_t)e.key >> 32); }
+
+/* heappush of q (its key is the routing key, >= 0) as the seq-th accepted request into the heap of n entries */
+__device__ __forceinline__ void hs_pq_push(hs_wring_entry *rg, uint32_t n, hs_wring_entry q, const uint32_t seq, const double *tab)
+{
+    q.key = (int64_t)(((uint64_t)seq << 32) | (uint64_t)(uint32_t)q.key);
+    const double p = hs_pq_prio(q, tab);
+    while (n > 0) {
+        const uint32_t up = (n - 1) >> 1;
+        const hs_wring_entry e = rg[up];
+        if (!hs_pq_less(p, seq, hs_pq_prio(e, tab), hs_pq_seq(e))) break;
+        rg[n] = e; n = up;
+    }
+    rg[n] = q;
+}
+
+/* heappop from the heap of n >= 1 entries: returns the root, its key the routing key again */
+__device__ __forceinline__ hs_wring_entry hs_pq_pop(hs_wring_entry *rg, const uint32_t n, const double *tab)
+{
+    hs_wring_entry top = rg[0];
+    top.key = (int32_t)top.key;
+    const uint32_t m = n - 1;
+    if (m > 0) {
+        const hs_wring_entry last = rg[m];
+        const double lp = hs_pq_prio(last, tab); const uint32_t ls = hs_pq_seq(last);
+        uint32_t pos = 0;
+        for (;;) {
+            uint32_t c = 2 * pos + 1;
+            if (c >= m) break;
+            hs_wring_entry ce = rg[c]; double cp = hs_pq_prio(ce, tab); uint32_t cs = hs_pq_seq(ce);
+            if (c + 1 < m) {
+                const hs_wring_entry re = rg[c + 1]; const double rp = hs_pq_prio(re, tab); const uint32_t rs = hs_pq_seq(re);
+                if (hs_pq_less(rp, rs, cp, cs)) { c = c + 1; ce = re; cp = rp; cs = rs; }
+            }
+            if (!hs_pq_less(cp, cs, lp, ls)) break;
+            rg[pos] = ce; pos = c;
+        }
+        rg[pos] = last;
+    }
+    return top;
+}
+
 #define HS_W_NCAP 24
 struct __align__(16) hs_wnow {          /* now-tier entry, 48 B */
     int64_t time; uint64_t idx; int64_t created; uint64_t aux;
@@ -99,6 +153,7 @@ struct hs_warp_model {
     const hs_profile_desc *profiles;
     const int32_t *sketch_tables;   /* per-key hash results of the SKETCH rows                */
     const double *key_cdf;          /* cumulative key probabilities of the Zipf sources       */
+    const double *profile_table;    /* STEP profile tables and the PriorityQueue servers' priority tables */
     uint64_t sk_total;              /* bytes of one replica's sketch states                   */
     uint32_t n_entities, n_cells, n_servers, fel_slots;   /* fel_slots = S, multiple of 32 */
     uint32_t block_bytes;           /* bytes of one replica block (multiple of 16)          */

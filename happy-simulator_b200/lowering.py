@@ -259,14 +259,49 @@ def _service(dist):
     raise UnsupportedModelError(f"service time distribution {name}")
 
 
-def _queue_policy(q):
+def _queue_policy(q, *, owner: str = "?", key_population: int = 0, priority: bool = False):
+    """-> (HS_Q_*, capacity or -1, priority table or None).  ``priority``: a PriorityQueue is lowered (Server rows);
+    its key must be a ``PriorityByKey`` whose table covers ``key_population``, the largest key population of the
+    model's sources."""
     pol = q.policy
     name = _cls(pol)
-    if name not in ("FIFOQueue", "LIFOQueue"):
+    if name not in ("FIFOQueue", "LIFOQueue") and not (priority and name == "PriorityQueue"):
         raise UnsupportedModelError(f"queue policy {name}")
     cap = pol.capacity
     cap = -1 if (isinstance(cap, float) and math.isinf(cap)) else int(cap)
-    return (A.HS_Q_LIFO if name == "LIFOQueue" else A.HS_Q_FIFO), cap
+    if name != "PriorityQueue":
+        return (A.HS_Q_LIFO if name == "LIFOQueue" else A.HS_Q_FIFO), cap, None
+    return A.HS_Q_PRIORITY, cap, _priority_table(getattr(pol, "_key", None), owner, key_population)
+
+
+def _priority_table(key, owner: str, key_population: int) -> list[float]:
+    """PriorityQueue._get_priority (queue_policy.py:245-253) as a table over the routing key."""
+    if key is None:
+        raise UnsupportedModelError(f"server {owner!r}: PriorityQueue without a key -- the reference falls back to "
+                                    "float(event), which raises TypeError on the first push; use "
+                                    "PriorityQueue(key=happysim_b200.PriorityByKey(values))")
+    if not getattr(key, "priority_by_routing_key", False):
+        raise UnsupportedModelError(f"server {owner!r}: PriorityQueue key {_cls(key)} is a Python callback and cannot run "
+                                    "on the device (use happysim_b200.PriorityByKey(values): priority = values[routing key])")
+    if key_population <= 0:
+        raise UnsupportedModelError(f"server {owner!r}: PriorityByKey reads the request's routing key, and no source of the "
+                                    "model draws one (context['metadata'] would be missing): use UniformKeyContext / "
+                                    "ZipfKeyContext")
+    values = list(key.values)
+    if len(values) < key_population:
+        raise UnsupportedModelError(f"server {owner!r}: PriorityByKey has {len(values)} values, the sources draw keys "
+                                    f"from {key_population}")
+    table = []
+    for k, v in enumerate(values):
+        if not isinstance(v, (int, float)):
+            raise UnsupportedModelError(f"server {owner!r}: priority of key {k} is a {type(v).__name__} (int, float or "
+                                        "bool only)")
+        if isinstance(v, int) and abs(v) > 1 << 53:
+            raise UnsupportedModelError(f"server {owner!r}: priority of key {k} ({v}) is an int a double cannot hold exactly")
+        if isinstance(v, float) and math.isnan(v):
+            raise UnsupportedModelError(f"server {owner!r}: priority of key {k} is NaN (it orders against nothing)")
+        table.append(float(v))
+    return table
 
 
 def fault_events(fault_schedule, sources, entities, probes):
@@ -392,6 +427,14 @@ def lower(sources, entities, *, key_population: int | None = None, probes=None, 
                 add(info.backend)
         i += 1
 
+    # the routing keys the model's requests carry: a PriorityByKey table must cover every one, and every request needs one
+    source_key_population, unkeyed = 0, []
+    for o in objs:
+        if kind_of(o) == A.HS_ENT_SOURCE:
+            pop_ = int(getattr(getattr(o._event_provider, "_context_fn", None), "key_population", 0) or 0)
+            source_key_population = max(source_key_population, pop_)
+            if pop_ <= 0:
+                unkeyed.append(getattr(o, "name", _cls(o)))
     b = ModelBuilder()
     pending_lb = []
     probe_rows = []
@@ -431,12 +474,17 @@ def lower(sources, entities, *, key_population: int | None = None, probes=None, 
             if _cls(cm) != "FixedConcurrency":
                 raise UnsupportedModelError(f"server {name!r}: concurrency model {_cls(cm)}")
             skind, mean = _service(o._service_time)
-            pol, cap = _queue_policy(o._queue)
+            pol, cap, prio = _queue_policy(o._queue, owner=name, key_population=source_key_population, priority=True)
+            if prio is not None and unkeyed:
+                raise UnsupportedModelError(f"server {name!r}: PriorityByKey reads the request's routing key, and source "
+                                            f"{unkeyed[0]!r} draws none (context['metadata'] would be missing)")
+            if prio is not None and faults:
+                raise UnsupportedModelError(f"server {name!r}: fault schedules do not run in a model with a PriorityQueue server")
             ds = o._downstream
             b.server(name, concurrency=int(cm.limit), mean_service_s=mean, exponential=(skind == A.HS_SVC_EXPONENTIAL),
-                     downstream=-1 if ds is None else ids[id(ds)], capacity=cap, lifo=(pol == A.HS_Q_LIFO))
+                     downstream=-1 if ds is None else ids[id(ds)], capacity=cap, lifo=(pol == A.HS_Q_LIFO), priorities=prio)
         elif k == A.HS_ENT_CACHE_SERVER:
-            pol, cap = _queue_policy(o._queue)
+            pol, cap, _ = _queue_policy(o._queue)
             if cap >= 0:
                 raise UnsupportedModelError(f"caching server {name!r}: bounded queue")
             pop = key_population or max((int(getattr(getattr(s_._event_provider, "_context_fn", None), "key_population", 0))

@@ -170,13 +170,14 @@ class FlatModel:
             d.cell_d0 = cd.ctypes.data_as(C.POINTER(C.c_double))
             d.cell_i0 = ci.ctypes.data_as(C.POINTER(C.c_int32))
             keep += [cd, ci]
+        if len(self.profile_table):                                  # STEP profile tables, PriorityQueue tables
+            pt = np.ascontiguousarray(self.profile_table, dtype=np.float64)
+            d.profile_table = pt.ctypes.data_as(C.POINTER(C.c_double))
+            d.n_profile_table = pt.shape[0]
+            keep.append(pt)
         if len(self.profiles):
             pr = np.array(self.profiles, dtype=A.PROFILE_DTYPE)          # a copy: p[2] of STEP rows is filled in below
             if len(self.profile_table):
-                pt = np.ascontiguousarray(self.profile_table, dtype=np.float64)
-                d.profile_table = pt.ctypes.data_as(C.POINTER(C.c_double))
-                d.n_profile_table = pt.shape[0]
-                keep.append(pt)
                 for row in pr:                                       # host address of the row's table, for the CPU oracle
                     if int(row["kind"]) == A.HS_PROF_STEP:
                         row["p"][2] = np.array([pt.ctypes.data + 8 * int(row["p"][0])], np.uint64).view(np.float64)[0]
@@ -245,11 +246,20 @@ class ModelBuilder:
                          key_population, i2, stop_after_ns, float(rate), i3=i3)
 
     def server(self, name="Server", *, concurrency=1, mean_service_s=0.01, exponential=True,
-               downstream=-1, capacity=-1, lifo=False):
-        return self._add(name, A.HS_ENT_SERVER, downstream, int(concurrency),
-                         A.HS_Q_LIFO if lifo else A.HS_Q_FIFO,
+               downstream=-1, capacity=-1, lifo=False, priorities=None):
+        """priorities: None (FIFOQueue, or LIFOQueue with lifo=True) or a PriorityQueue's table, one priority per
+        routing key (floats; lower leaves first, ties in insertion order).  The table is appended to profile_table and
+        the row's i3 is 1 + its offset there (include/hs_b200.h)."""
+        pol, i3 = (A.HS_Q_LIFO if lifo else A.HS_Q_FIFO), 0
+        if priorities is not None:
+            if lifo:
+                raise ValueError("a server has one queue policy: lifo or priorities")
+            pol = A.HS_Q_PRIORITY
+            i3 = 1 + sum(len(t) for t in self._profile_tables)
+            self._profile_tables.append([float(x) for x in priorities])
+        return self._add(name, A.HS_ENT_SERVER, downstream, int(concurrency), pol,
                          A.HS_SVC_EXPONENTIAL if exponential else A.HS_SVC_CONSTANT,
-                         int(capacity), float(mean_service_s))
+                         int(capacity), float(mean_service_s), i3=i3)
 
     def cache_server(self, name="CachingServer", *, key_slots, cache_ttl_s=30.0, cache_read_latency_s=0.0001,
                      datastore_read_latency_s=0.005, processing_latency_s=0.001, lifo=False):
@@ -379,8 +389,8 @@ class ModelBuilder:
                       key_table=self._key_table)
         if self._profiles:
             m.profiles = np.array(self._profiles, dtype=A.PROFILE_DTYPE)
-            if self._profile_tables:
-                m.profile_table = np.array([x for t in self._profile_tables for x in t], dtype=np.float64)
+        if self._profile_tables:
+            m.profile_table = np.array([x for t in self._profile_tables for x in t], dtype=np.float64)
         if self._sketch_tables:
             m.sketch_tables = np.concatenate([t.ravel() for t in self._sketch_tables]).astype(np.int32)
         if self._key_cdf:

@@ -331,6 +331,16 @@ class ParallelSimulation:
         for q in range(len(parts)):
             for l in out_links[q]:
                 models[l.dest].inbox_cap = self.link_buffer * max(1, sum(1 for qq in range(len(parts)) for x in out_links[qq] if x.dest == l.dest))
+        # a PriorityQueue server in a partition that receives over a link may see the keys of every partition's sources
+        pops = [int(m.entities["i1"][i]) for m in models for i in m.ids_of(A.HS_ENT_SOURCE)
+                if int(m.entities["kind"][int(m.entities["target"][i])]) != A.HS_ENT_PROBE]
+        for d, m in enumerate(models):
+            for i in m.ids_of(A.HS_ENT_SERVER) if m.inbox_cap else ():
+                if int(m.entities["i1"][i]) == A.HS_Q_PRIORITY and \
+                        (min(pops, default=0) <= 0 or len(objects[d][i]._queue.policy._key.values) < max(pops)):
+                    raise UnsupportedModelError(f"server '{getattr(objects[d][i], 'name', '?')}' in partition '{names[d]}': "
+                                                "its PriorityByKey table must cover the routing keys of every partition's "
+                                                "sources, and every source must draw one")
         self._linked = LinkedModel(models, names, out_links, window_s=window, n_streams=max(1, len(streams)), objects=objects)
         self._linked.validate()
         self._linked.window_ends(self._end_ns)      # raises if the coordinator's clock could not reach the end time

@@ -122,6 +122,8 @@ def write_back(model, objects, out, r: int, instant_cls) -> None:
                 o._event_provider._generated = int(row["c1"])
         elif k == A.HS_ENT_SERVER:
             o._queue.stats_accepted, o._queue.stats_dropped = int(row["c0"]), int(row["c1"])
+            if int(model.entities["i1"][i]) == A.HS_Q_PRIORITY:      # PriorityQueue._insert_counter: successful pushes
+                o._queue.policy._insert_counter = int(row["c0"])
             o._requests_completed, o._requests_rejected = int(row["c2"]), int(row["c3"])
             o._total_service_time = float(row["f0"])
             o._service_times = per_server[i]

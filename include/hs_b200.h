@@ -103,7 +103,9 @@ enum { HS_METRIC_DEPTH = 0, HS_METRIC_ACTIVE_REQUESTS = 1, HS_METRIC_UTILIZATION
        HS_METRIC_GENERATED_COUNT = 8 };
 enum { HS_ARR_CONSTANT = 0, HS_ARR_POISSON = 1 };       /* load/providers/{constant,poisson}_arrival.py */
 enum { HS_SVC_CONSTANT = 0, HS_SVC_EXPONENTIAL = 1 };   /* distributions/{constant,exponential}.py      */
-enum { HS_Q_FIFO = 0, HS_Q_LIFO = 1 };                  /* components/queue_policy.py:75,117            */
+enum { HS_Q_FIFO = 0, HS_Q_LIFO = 1,                   /* components/queue_policy.py:75,117            */
+       HS_Q_PRIORITY = 2 };  /* queue_policy.py:189-287 PriorityQueue(key=happysim_b200.PriorityByKey(values)): pops the
+                                smallest (values[routing key], insertion order); SERVER rows only, see hs_entity_desc.i3 */
 enum { HS_LB_ROUND_ROBIN = 0, HS_LB_KEY_TABLE = 1 };    /* strategies.py:50 RoundRobin, :336 ConsistentHash
                                                            (ring lookup precomputed per key on the host) */
 
@@ -129,7 +131,7 @@ typedef struct hs_entity_desc {
     int32_t kind;      /* HS_ENT_*                                                              */
     int32_t target;    /* SOURCE: entity receiving payloads; SERVER: downstream or -1; PROBE: measured entity */
     int32_t i0;        /* SOURCE: HS_ARR_*; SERVER: concurrency (FixedConcurrency); LB: HS_LB_*; PROBE: HS_METRIC_* */
-    int32_t i1;        /* SOURCE: key population (0 = no routing key); SERVER: HS_Q_*;
+    int32_t i1;        /* SOURCE: key population (0 = no routing key); SERVER: HS_Q_* (CACHE_SERVER: FIFO or LIFO);
                           LB: offset of its backend list in hs_model_desc.backends;
                           SKETCH: offset of its table in hs_model_desc.sketch_tables            */
     int32_t i2;        /* SOURCE: routing-key distribution: 0 = uniform (distributions/uniform.py:57), k > 0 = Zipf with
@@ -138,7 +140,12 @@ typedef struct hs_entity_desc {
                           | TDIGEST buffer size int(compression * 2), tdigest.py:88 */
     int32_t i3;        /* SOURCE: 0 = ConstantRateProfile(d0); k > 0 = profiles[k - 1] (non-constant
                           rate profile, general arrival path); SKETCH: CMS width | BLOOM size_bits
-                          | TDIGEST centroid capacity (>= 2 x buffer size); others: reserved, 0 */
+                          | TDIGEST centroid capacity (>= 2 x buffer size);
+                          SERVER with HS_Q_PRIORITY: 1 + offset in hs_model_desc.profile_table of its priority table, one
+                          double per routing key (priority of key k = table[k]; no NaN), covering the key population of
+                          every SOURCE row; every SOURCE row that sends requests (all but a Probe's ticking) must draw
+                          keys -- a request without one has no priority, the reference's key raises.  The lane engine
+                          does not run such a model.  Other SERVER rows: 0; others: reserved, 0 */
     int64_t l0;        /* SOURCE: stop_after in ns or -1; SERVER: queue capacity or -1 (= inf);
                           SKETCH: key population K = row stride of its table in sketch_tables; 0 = no per-key
                           table: the device evaluates the SHA-256 hashes per event (any key population) and
@@ -185,7 +192,9 @@ typedef struct hs_model_desc {
     const double *key_cdf;
     /* Tables of the piecewise-constant (STEP) rate profiles: for a profile with n breakpoints, n ascending
      * breakpoints (seconds) followed by n + 1 rates; rate(t) = rates[#{breakpoints <= t}].  A user-defined
-     * Profile.get_rate that is a step function (examples/queuing/m_m_1_queue.py:104-169) lowers to one. */
+     * Profile.get_rate that is a step function (examples/queuing/m_m_1_queue.py:104-169) lowers to one.
+     * The priority tables of HS_Q_PRIORITY servers (one double per routing key, see hs_entity_desc.i3) are appended
+     * to the same array. */
     const double *profile_table;
     uint64_t n_profile_table;      /* total length of profile_table[]                          */
 } hs_model_desc;
@@ -221,7 +230,7 @@ typedef struct hs_run_params {
     uint32_t sample_cap;       /* Sink-sample ring entries per replica                         */
     uint32_t service_cap;      /* service-time ring entries per replica                        */
     uint32_t queue_ring;       /* device queue ring entries per server (power of two), 0 = default */
-    uint32_t engine;           /* 0 auto, 1 warp engine (general), 2 lane engine (single server), 3 thread engine (general) */
+    uint32_t engine;           /* 0 auto, 1 warp engine (general), 2 lane engine (single FIFO / LIFO server), 3 thread engine (general) */
     /* Windowed execution (reference: Simulation._run_window, core/simulation.py:527-541):
      * when 0 <= window_end_ns < end_ns the call pauses every replica before the first
      * event later than window_end_ns and keeps its state on the device; a following
