@@ -100,12 +100,12 @@ def _at_window_end(lm, end_ns, k):
 def _grid_tie_schedule(lm, end_s):
     """B's first delivered request, found on the fault-free run of the fault oracle: a crash of B.server at its time,
     with its sort index (the fault events before it, one index each, lie beyond end_time)"""
-    import linked_fault_oracle_lib as FO
+    import layered_oracle_lib as LO
     import oracle_lib as O
     end_ns = int(end_s * 1e9)
     ps = [O.make_params(seed=3, end_ns=end_ns, rid_base=q, rid_stride=3, record_cap=4096, sample_cap=16, service_cap=16)
           for q in range(2)]
-    outs, *_ = FO.run_linked(lm, ps, end_ns=end_ns, cseed=3)
+    outs, *_ = LO.run_linked(lm, ps, end_ns=end_ns, cseed=3)
     rec = outs[1]["records"][0]
     first = rec[rec["kind"] == A.HS_EV_REQ_ENQUEUE][0]
     t_ns, idx = int(first["time_ns"]), int(first["sort_index"])

@@ -1,9 +1,13 @@
-"""ctypes binding of the CPU oracle (oracle/libhs_oracle.so).  Test infrastructure."""
+"""ctypes binding of the CPU oracle (oracle/libhs_oracle.so), and the one way the tests build and call the other host
+libraries they check against (build, run_range_parallel, run_linked_on, run_slices).  Test infrastructure."""
 from __future__ import annotations
 
 import ctypes as C
+import hashlib
 import os
+import re
 import subprocess
+import tempfile
 
 import numpy as np
 
@@ -68,6 +72,43 @@ def lib():
     return _lib
 
 
+_INCLUDE = re.compile(rb'^[ \t]*#[ \t]*include[ \t]*"([^"]+)"', re.M)
+_built: dict = {}
+
+
+def _sources(path: str, seen: dict) -> dict:
+    """{path: contents} of ``path`` and of every file it includes with quotes, transitively"""
+    path = os.path.normpath(path)
+    if path not in seen:
+        seen[path] = data = open(path, "rb").read()
+        for inc in _INCLUDE.findall(data):
+            _sources(os.path.join(os.path.dirname(path), inc.decode()), seen)
+    return seen
+
+
+def build(src: str, defines=()) -> C.CDLL:
+    """``src`` (a path under the repository) compiled by oracle/Makefile's rule, with ``-D`` for each of ``defines``,
+    and loaded.  The library goes to a per-user temporary directory, under a name keyed by every file ``src``
+    includes, the Makefile and the defines, so the repository tree stays as it is and an edit rebuilds it."""
+    key = (src, tuple(defines))
+    if key not in _built:
+        src, mk = os.path.join(_ROOT, src), os.path.join(_ROOT, "oracle", "Makefile")
+        h = hashlib.sha256()
+        for data in _sources(src, {mk: open(mk, "rb").read()}).values():
+            h.update(data)
+        h.update(repr(key[1]).encode())
+        d = os.path.join(tempfile.gettempdir(), f"hs_oracle_{os.getuid()}")
+        os.makedirs(d, exist_ok=True)
+        so = os.path.join(d, f"lib{os.path.splitext(os.path.basename(src))[0]}_{h.hexdigest()[:16]}.so")
+        if not os.path.exists(so):
+            tmp = f"{so}.{os.getpid()}"
+            subprocess.check_call(["make", "-s", "-f", mk, f"SRC={src}", f"OUT={tmp}",
+                                   "DEFS=" + " ".join(f"-D{x}" for x in defines)])
+            os.replace(tmp, so)
+        _built[key] = C.CDLL(so)
+    return _built[key]
+
+
 def alloc_outputs(n_entities: int, p: A.RunParams, sketch_bytes: int = 0):
     """Host buffers (numpy) + the hs_outputs struct pointing at them."""
     n = p.n_replicas
@@ -114,23 +155,41 @@ def _pool_map(fn, items):
         return list(ex.map(fn, items))
 
 
-def oracle_run_parallel(model: happysim_b200.FlatModel, p: A.RunParams, chunk: int = 256):
-    """oracle_run on a thread pool: hs_oracle_run_range over slices of ``chunk`` replicas into one set of buffers
-    (ctypes releases the GIL for the call, and a replica only writes its own rows)."""
+def run_range_parallel(fn, model: happysim_b200.FlatModel, p: A.RunParams, chunk: int = 256, *extra):
+    """``fn`` -- hs_oracle_run_range or an entry point with its arguments, then ``extra`` -- on a thread pool over
+    slices of ``chunk`` replicas into one set of buffers (ctypes releases the GIL for the call, and a replica only
+    writes its own rows)."""
     d = model.desc()
     bufs, o = alloc_outputs(model.n_entities, p, model.sketch_layout()[2])
     n = p.n_replicas
 
     def part(r0):
-        assert lib().hs_oracle_run_range(C.byref(d), C.byref(p), C.byref(o), r0, min(n, r0 + chunk)) == 0
+        assert fn(C.byref(d), C.byref(p), C.byref(o), r0, min(n, r0 + chunk), *extra) == 0
 
     _pool_map(part, range(0, n, chunk))
     return bufs
 
 
-def oracle_run_linked_parallel(lm, params: list, *, end_ns, cseed, chunk: int = 64):
-    """oracle_run_linked on a thread pool: slices of ``chunk`` replicas (replica_index_base moved along, so every
-    replica keeps its global index and therefore its draws), concatenated in replica order."""
+def oracle_run_parallel(model: happysim_b200.FlatModel, p: A.RunParams, chunk: int = 256):
+    """oracle_run on a thread pool: hs_oracle_run_range over slices of ``chunk`` replicas."""
+    return run_range_parallel(lib().hs_oracle_run_range, model, p, chunk)
+
+
+def _cat(xs):
+    """the per-replica results of consecutive slices joined: arrays concatenated, lists and dicts of them item by item"""
+    if xs[0] is None:
+        return None
+    if isinstance(xs[0], dict):
+        return {k: _cat([x[k] for x in xs]) for k in xs[0]}
+    if isinstance(xs[0], list):
+        return [_cat([x[q] for x in xs]) for q in range(len(xs[0]))]
+    return np.concatenate(xs)
+
+
+def run_slices(run, params: list, chunk: int):
+    """``run(ps)`` of a linked run on a thread pool over slices of ``chunk`` replicas (``ps``: ``params`` with
+    replica_index_base moved along, so every replica keeps its global index and with it its draws and its cell).  What
+    ``run`` returns, every item per replica, is concatenated in replica order."""
     n = params[0].n_replicas
 
     def part(r0):
@@ -139,42 +198,55 @@ def oracle_run_linked_parallel(lm, params: list, *, end_ns, cseed, chunk: int = 
             q = A.RunParams.from_buffer_copy(p)
             q.n_replicas, q.replica_index_base = min(n, r0 + chunk) - r0, p.replica_index_base + r0
             ps.append(q)
-        return oracle_run_linked(lm, ps, end_ns=end_ns, cseed=cseed)
+        return run(ps)
 
     parts = _pool_map(part, range(0, n, chunk))
-    outs = [{k: (None if v is None else np.concatenate([pt[0][q][k] for pt in parts])) for k, v in parts[0][0][q].items()}
-            for q in range(lm.n_partitions)]
-    return outs, np.concatenate([pt[1] for pt in parts]), np.concatenate([pt[2] for pt in parts]), parts[0][3]
+    return [_cat([pt[i] for pt in parts]) for i in range(len(parts[0]))]
 
 
-def oracle_run_linked(lm, params: list, *, end_ns, cseed, cseed_stride=0, crid_base=None, crid_stride=None):
-    """A linked run (happysim_b200.linked.LinkedModel) on the oracle: per partition the usual output buffers,
-    plus per-replica counts of delivered / lost cross-partition events."""
-    L = lib()
+def run_linked_on(fn, lm, params: list, *, end_ns, cseed, cseed_stride=0, crid_base=None, crid_stride=None,
+                  replicas_per_cell=None, hw_rows=None):
+    """``fn`` -- hs_oracle_run_linked or an entry point with its arguments -- on a linked run
+    (happysim_b200.linked.LinkedModel): per partition the usual output buffers, per replica the delivered / lost
+    cross-partition events, and the window ends.  Partition q runs ``params[q]``; the coordinator draws with key
+    ``cseed + g * cseed_stride`` and replica word ``crid_base + g * crid_stride`` (default P and P + 1, LinkedRun's).
+    Where ``fn`` takes them: ``replicas_per_cell`` passes the cell table (every partition's link count, the cells,
+    replicas per cell) after the link destinations, ``hw_rows`` (a uint32 array per partition) goes last."""
     nP = lm.n_partitions
     descs = [m.desc() for m in lm.models]
     outs = [alloc_outputs(m.n_entities, p, m.sketch_layout()[2]) for m, p in zip(lm.models, params)]
     ends = np.array(lm.window_ends(end_ns), dtype=np.int64)
-    link_arrs, dst_arrs = [], []
-    for q in range(nP):
-        arr, dst = lm.link_descs(q)
-        link_arrs.append(arr)
-        dst_arrs.append((C.c_uint32 * max(1, len(dst)))(*dst))
-    PP = lambda T, xs: (C.POINTER(T) * nP)(*[C.cast(C.pointer(x) if not isinstance(x, C.Array) else x, C.POINTER(T)) for x in xs])
+    link_arrs, dsts = zip(*(lm.link_descs(q) for q in range(nP)))
+    dst_arrs = [(C.c_uint32 * max(1, len(d)))(*d) for d in dsts]
+    PP = lambda T, xs: (C.POINTER(T) * nP)(*[C.cast(x if isinstance(x, C.Array) else C.pointer(x), C.POINTER(T)) for x in xs])  # noqa: E731
     n = params[0].n_replicas
     delivered, lost = np.zeros(n, np.uint64), np.zeros(n, np.uint64)
-    L.hs_oracle_run_linked.restype = C.c_int
-    L.hs_oracle_run_linked.argtypes = [C.c_uint32, C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p,
-                                       C.POINTER(C.c_int64), C.c_uint32, C.c_uint32, C.c_uint64, C.c_uint64, C.c_uint32,
-                                       C.c_uint32, C.POINTER(C.c_uint64), C.POINTER(C.c_uint64)]
-    rc = L.hs_oracle_run_linked(nP, PP(A.ModelDesc, descs), PP(A.RunParams, params), PP(A.Outputs, [o for _, o in outs]),
-                                PP(A.LinkDesc, link_arrs), PP(C.c_uint32, dst_arrs),
-                                ends.ctypes.data_as(C.POINTER(C.c_int64)), len(ends), lm.n_streams,
-                                cseed, cseed_stride, nP if crid_base is None else crid_base,
-                                nP + 1 if crid_stride is None else crid_stride,
-                                delivered.ctypes.data_as(C.POINTER(C.c_uint64)), lost.ctypes.data_as(C.POINTER(C.c_uint64)))
+    u32, u64 = C.c_uint32, C.c_uint64
+    args = [u32(nP), PP(A.ModelDesc, descs), PP(A.RunParams, params), PP(A.Outputs, [o for _, o in outs]),
+            PP(A.LinkDesc, link_arrs), PP(C.c_uint32, dst_arrs)]
+    if replicas_per_cell is not None:
+        args += [(C.c_uint32 * nP)(*[len(ls) for ls in lm.links]), u32(max(1, lm.n_cells)), u32(max(1, int(replicas_per_cell)))]
+    args += [ends.ctypes.data_as(C.POINTER(C.c_int64)), u32(len(ends)), u32(lm.n_streams), u64(cseed), u64(cseed_stride),
+             u32(nP if crid_base is None else crid_base), u32(nP + 1 if crid_stride is None else crid_stride),
+             delivered.ctypes.data_as(C.POINTER(C.c_uint64)), lost.ctypes.data_as(C.POINTER(C.c_uint64))]
+    if hw_rows is not None:
+        args.append((C.POINTER(C.c_uint32) * nP)(*[r.ctypes.data_as(C.POINTER(C.c_uint32)) for r in hw_rows]))
+    rc = fn(*args)
     assert rc == 0, rc
     return [b for b, _ in outs], delivered, lost, ends
+
+
+def oracle_run_linked_parallel(lm, params: list, *, end_ns, cseed, chunk: int = 64):
+    """oracle_run_linked on a thread pool (run_slices)."""
+    outs, delivered, lost = run_slices(lambda ps: oracle_run_linked(lm, ps, end_ns=end_ns, cseed=cseed)[:3], params, chunk)
+    return outs, delivered, lost, np.array(lm.window_ends(end_ns), dtype=np.int64)
+
+
+def oracle_run_linked(lm, params: list, *, end_ns, cseed, cseed_stride=0, crid_base=None, crid_stride=None):
+    """A linked run (happysim_b200.linked.LinkedModel) on the oracle: per partition the usual output buffers,
+    plus per-replica counts of delivered / lost cross-partition events (run_linked_on)."""
+    return run_linked_on(lib().hs_oracle_run_linked, lm, params, end_ns=end_ns, cseed=cseed, cseed_stride=cseed_stride,
+                         crid_base=crid_base, crid_stride=crid_stride)
 
 
 class OracleLinkedRun:

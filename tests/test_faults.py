@@ -125,8 +125,8 @@ def test_reference_schedule_lowers_like_the_mirror():
     assert a.tobytes() == b.tobytes()
 
 
-# ---- the fault oracle (tests/fault_oracle.c) against the reference ----------------------------------------------------
-import fault_oracle_lib as FO  # noqa: E402
+# ---- the fault oracle (tests/layered_oracle.c) against the reference ----------------------------------------------------
+import layered_oracle_lib as LO  # noqa: E402
 
 
 def _check_ref(ref, got, r=0):
@@ -142,7 +142,7 @@ def _check_ref(ref, got, r=0):
 @pytest.mark.parametrize("name", G.case_names("fault_"))
 def test_fault_oracle_reproduces_reference_fixture(name):
     model, kw, z = G.load(name)
-    got = FO.run(model, engine.make_params(n_replicas=1, **G.caps(z), **kw))
+    got = LO.run(model, engine.make_params(n_replicas=1, **G.caps(z), **kw))
     G.check_against(z, got)
     tie = bool(int(got["summaries"]["status"][0]) & A.HS_ST_FAULT_TIE)
     assert tie == name.startswith("fault_tie"), "HS_ST_FAULT_TIE exactly where the reference tied"
@@ -184,7 +184,7 @@ def _oracle_vs_reference(version, seed):
     model, build, kw, plan, cancel = reference_case_kw(version, seed, seed % 5)
     fm, ref, meta = GF.run_case(model, build, kw)
     assert with_faults(model, plan, cancel).entities.tobytes() == fm.entities.tobytes()
-    got = FO.run(fm, engine.make_params(n_replicas=1, seed=kw["seed"], rid_base=seed % 5, end_ns=int(kw["end_s"] * 1e9),
+    got = LO.run(fm, engine.make_params(n_replicas=1, seed=kw["seed"], rid_base=seed % 5, end_ns=int(kw["end_s"] * 1e9),
                                         record_cap=len(ref["records"]) + 1, sample_cap=len(ref["sink_samples"]) + 1,
                                         service_cap=len(ref["service_samples"]) + 1))
     _check_ref(ref, got)
@@ -260,7 +260,7 @@ def test_random_fault_fixture_covers_every_seed():
 def test_fault_oracle_reproduces_random_fault_fixture(version, seed):
     model, end_s, plan, cancel, run_seed, what, _ = random_fault_case(version, seed)
     fm = with_faults(model, plan, cancel)
-    got = FO.run(fm, engine.make_params(n_replicas=1, seed=run_seed, end_ns=int(end_s * 1e9)))
+    got = LO.run(fm, engine.make_params(n_replicas=1, seed=run_seed, end_ns=int(end_s * 1e9)))
     check_random_fault_reference(fm, version, seed, got)
 
 
@@ -296,7 +296,7 @@ def test_demultiplex_leaves_out_requests_a_crashed_sink_dropped(version, seed):
     from happysim_b200 import results
     model, end_s, plan, cancel, run_seed, what, _ = random_fault_case(version, seed)
     fm = with_faults(model, plan, cancel)
-    out = FO.run(fm, engine.make_params(seed=run_seed, end_ns=int(end_s * 1e9), n_replicas=8, rid_stride=1,
+    out = LO.run(fm, engine.make_params(seed=run_seed, end_ns=int(end_s * 1e9), n_replicas=8, rid_stride=1,
                                         record_cap=16384, sample_cap=4096, service_cap=4096))
     assert int(out["summaries"]["events_processed"].max()) < 16384
     collectors = fm.ids_of(A.HS_ENT_SINK) + fm.ids_of(A.HS_ENT_PROBE)
@@ -317,6 +317,6 @@ def test_some_multi_collector_models_drop_requests_at_a_crashed_sink():
     for version, seed in _multi_collector_cases():
         model, end_s, plan, cancel, run_seed, _, _ = random_fault_case(version, seed)
         fm = with_faults(model, plan, cancel)
-        out = FO.run(fm, engine.make_params(seed=run_seed, end_ns=int(end_s * 1e9), n_replicas=1, record_cap=16384))
+        out = LO.run(fm, engine.make_params(seed=run_seed, end_ns=int(end_s * 1e9), n_replicas=1, record_cap=16384))
         n += int(_dropped_by_replay(fm, out["records"][0][: int(out["summaries"]["events_processed"][0])]).sum())
     assert n > 0

@@ -1,12 +1,12 @@
 """Node faults (CrashNode, PauseNode) on the device: both general engines against the fixtures recorded from the
-unmodified reference (tests/golden/fault_*.npz), larger ensembles against the fault oracle (tests/fault_oracle.c) on
+unmodified reference (tests/golden/fault_*.npz), larger ensembles against the fault oracle (tests/layered_oracle.c) on
 every replica, windowed runs cut between a crash and its restart, ties, install() and the mirror's write-back."""
 import random
 
 import numpy as np
 import pytest
 
-import fault_oracle_lib as FO
+import layered_oracle_lib as LO
 import golden_lib as G
 import happysim_b200 as hs
 from happysim_b200 import engine, _abi as A
@@ -66,7 +66,7 @@ def test_ensembles_match_the_fault_oracle_on_every_replica(eng, n):
     m = _farm_with_faults()
     eng.upload(m)
     kw = dict(seed=9, end_ns=8 * 10**9, n_replicas=n, record_cap=512, sample_cap=256, service_cap=256)
-    want = FO.run(m, engine.make_params(**kw))
+    want = LO.run(m, engine.make_params(**kw))
     for e in (3, 1):
         eng.run(engine.make_params(engine=e, **kw))
         got = eng.read_outputs(); li = eng.last_launch()
@@ -87,7 +87,7 @@ def test_mixed_fixture_ensemble_matches_the_fault_oracle_and_is_tie_free(eng):
     eng.upload(model)
     kw = dict(kw); kw.pop("rid_base")
     p = dict(n_replicas=1024, rid_stride=1, record_cap=1024, sample_cap=512, service_cap=512, **kw)
-    want = FO.run(model, engine.make_params(**p))
+    want = LO.run(model, engine.make_params(**p))
     assert int(want["summaries"]["status"].max()) == 0
     for e in (1, 3):
         eng.run(engine.make_params(engine=e, **p))

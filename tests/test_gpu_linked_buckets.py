@@ -296,7 +296,7 @@ def test_tandem_heavy_100s_at_16384_replicas():
 # ---- the reference fixtures (tests/golden/gen_linked_bucket_golden.py) ----------------------------------------------
 
 import linked_bucket_models as LB  # noqa: E402
-import linked_fault_oracle_lib as FO  # noqa: E402
+import layered_oracle_lib as LO  # noqa: E402
 import oracle_lib as O  # noqa: E402
 
 
@@ -313,7 +313,7 @@ def test_run_ensemble_equals_the_reference_and_the_oracle(name):
     nP = lm.n_partitions
     params = [O.make_params(seed=kw["seed"], end_ns=kw["end_ns"], n_replicas=n, rid_base=q, rid_stride=nP + 1,
                             record_cap=8192, sample_cap=4096, service_cap=4096) for q in range(nP)]
-    run = FO.run_linked if any(m.ids_of(A.HS_ENT_FAULT) for m in lm.models) else O.oracle_run_linked
+    run = LO.run_linked if any(m.ids_of(A.HS_ENT_FAULT) for m in lm.models) else O.oracle_run_linked
     want, wd, wl, _ = run(lm, params, end_ns=kw["end_ns"], cseed=kw["seed"])
     assert (delivered == wd).all() and (lost == wl).all()
     rows = 0

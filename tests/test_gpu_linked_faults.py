@@ -1,11 +1,11 @@
 """Node faults in the partitions of a linked ParallelSimulation, on the device: the thread engine's LINKED | FAULTS
 instantiations against the fixtures recorded from the unmodified reference (tests/golden/lfault_*.npz), ensembles
-against the linked fault oracle (tests/linked_fault_oracle.c) on every replica, the random models, and the mirror's
+against the linked fault oracle (tests/layered_oracle.c) on every replica, the random models, and the mirror's
 ParallelSimulation.run() / run_ensemble()."""
 import numpy as np
 import pytest
 
-import linked_fault_oracle_lib as FO
+import layered_oracle_lib as LO
 import golden_lib as G
 import happysim_b200 as hs
 import linked_fault_models as LF
@@ -101,7 +101,7 @@ def test_ensembles_match_the_linked_fault_oracle_on_every_replica(n):
         outs, (delivered, lost, over), infos = _launches(run, n, seed, end_ns, caps)
     finally:
         run.close()
-    want, wd, wl, ends = FO.run_linked_parallel(lm, _params(lm, seed, end_ns, n, caps), end_ns=end_ns, cseed=seed)
+    want, wd, wl, ends = LO.run_linked_parallel(lm, _params(lm, seed, end_ns, n, caps), end_ns=end_ns, cseed=seed)
     assert not over.any()
     assert (delivered == wd).all() and (lost == wl).all()
     for q, info in enumerate(infos):
@@ -133,7 +133,7 @@ def test_random_linked_fault_models_on_the_device():
             outs, (delivered, lost, over), infos = _launches(run, 6, 1000 + seed, end_ns, caps)
         finally:
             run.close()
-        want, wd, wl, _ = FO.run_linked(lm, _params(lm, 1000 + seed, end_ns, 6, caps), end_ns=end_ns, cseed=1000 + seed)
+        want, wd, wl, _ = LO.run_linked(lm, _params(lm, 1000 + seed, end_ns, 6, caps), end_ns=end_ns, cseed=1000 + seed)
         tie = np.zeros(6, bool)
         for q in range(lm.n_partitions):
             tie |= (outs[q]["summaries"]["status"] & (A.HS_ST_LINK_TIE | A.HS_ST_FAULT_TIE)) != 0

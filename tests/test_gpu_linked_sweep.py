@@ -1,5 +1,5 @@
 """Linked ParallelSimulations as the cells of one ensemble, on the device: every replica of celled linked runs against
-the cell oracle (tests/linked_sweep_oracle.c) -- random linked models with per-cell model rows and per-cell link latency
+the cell oracle (tests/layered_oracle.c) -- random linked models with per-cell model rows and per-cell link latency
 and loss, node faults, replicas_per_cell > 1, a nonzero replica_index_base -- the celled ensemble against each cell's own
 ensemble, time buckets per cell, run_sweep over linked configurations, shards, and a sweep-sized point."""
 import numpy as np
@@ -7,6 +7,7 @@ import pytest
 
 import golden_lib as G
 import happysim_b200 as hs
+import layered_oracle_lib as LO
 import linked_fault_models as LF
 import linked_sweep_lib as LS
 import random_models as RM
@@ -34,7 +35,7 @@ def _device(lm, *, seed, end_ns, n, caps=CAPS, base=0, rpc=1, seed_stride=0, rid
 
 def _oracle(lm, *, seed, end_ns, n, caps=CAPS, base=0, rpc=1):
     ps = LS.partition_params(lm, seed=seed, end_ns=end_ns, n=n, caps=caps, replica_index_base=base, replicas_per_cell=rpc)
-    return LS.run_cells_parallel(lm, ps, end_ns=end_ns, cseed=seed, replicas_per_cell=rpc)
+    return LO.run_linked_parallel(lm, ps, end_ns=end_ns, cseed=seed, replicas_per_cell=rpc)
 
 
 def _check(lm, *, seed, end_ns, n, base, rpc, grid=False):

@@ -1,5 +1,5 @@
 """PriorityQueue servers on the device: the binary heap in each server's queue ring (csrc/hs_warp_engine.cuh, hs_pq_push /
-hs_pq_pop), on both general engines, against the priority oracle (tests/priority_oracle.c) for every replica and the
+hs_pq_pop), on both general engines, against the priority oracle (tests/layered_oracle.c) for every replica and the
 unmodified reference's fixtures for the fixture's replica -- event records, order hashes, Sink samples, service times
 and statistics, bit for bit, with recorder rings that wrap.  Also: runs cut into windows that resume with non-empty
 heaps, the thread engine's kernels by ensemble size, a queue ring that starts too small and grows, the engine choice,
@@ -11,7 +11,7 @@ import golden_lib as G
 import happysim_b200 as hs
 import oracle_lib as O
 import priority_models as PM
-import priority_oracle_lib as PO
+import layered_oracle_lib as LO
 from happysim_b200 import _abi as A, engine
 from happysim_b200.linked import LinkedRun
 from test_gpu_lane_parity import assert_same
@@ -45,10 +45,10 @@ def test_fixture_on_the_general_engines(eng, name, eng_id):
     eng.run(p)
     got = eng.read_outputs()
     G.check_against(z, got, 0)
-    assert_same(got, PO.run(model, p))
+    assert_same(got, LO.run(model, p))
     p = O.make_params(seed=kw["seed"], end_ns=kw["end_ns"], n_replicas=6, queue_ring=256, engine=eng_id, **WRAP)
     eng.run(p)
-    got, want = eng.read_outputs(), PO.run(model, p)
+    got, want = eng.read_outputs(), LO.run(model, p)
     assert np.all(want["summaries"]["events_processed"] > WRAP["record_cap"])          # the rings wrap
     assert_same(got, want)
 
@@ -61,7 +61,7 @@ def test_fixture_cut_into_windows(eng, name, eng_id):
     end_ns = kw["end_ns"]
     cuts = [end_ns // 5 + 7, end_ns // 2 + 3, (4 * end_ns) // 5]
     base = dict(seed=kw["seed"], n_replicas=5, queue_ring=256, **WRAP)
-    want = PO.run(model, O.make_params(end_ns=end_ns, **base))
+    want = LO.run(model, O.make_params(end_ns=end_ns, **base))
     eng.upload(model)
     eng.run(engine.make_params(end_ns=end_ns, window_end_ns=cuts[0], engine=eng_id, **base))
     for c in cuts[1:]:
@@ -75,7 +75,7 @@ def test_random_model_on_every_general_engine(eng, seed):
     model, end_s, _ = PM.random_priority_model(seed)
     kw = dict(seed=int(RANDOM["base_seed"]) + seed, end_ns=int(end_s * 1e9), n_replicas=5, record_cap=12000,
               sample_cap=1500, service_cap=1500, queue_ring=1024)
-    want = PO.run(model, O.make_params(**kw))
+    want = LO.run(model, O.make_params(**kw))
     ws = RANDOM[f"s{seed}_summary"][0]
     for f in ("events_processed", "order_hash", "n_sink_samples", "n_service_samples"):
         assert int(want["summaries"][0][f]) == int(ws[f])
@@ -104,7 +104,7 @@ def test_thread_engine_kernels(eng, sm, row):
     eng.run(engine.make_params(engine=3, **p))
     check_thread_geometry(eng.last_launch(), row, n)
     got = eng.read_outputs()
-    want = PO.run(model, O.make_params(**p), chunk=1024)
+    want = LO.run(model, O.make_params(**p), chunk=1024)
     assert not (want["summaries"]["status"] & A.HS_ST_QUEUE_OVERFLOW).any()
     assert_same(got, want)
 
@@ -190,7 +190,7 @@ def test_linked_partition_with_a_priority_server():
     finally:
         run.close()
     params = [O.make_params(seed=11, end_ns=end_ns, n_replicas=n, rid_base=q, rid_stride=nP + 1, **caps[q]) for q in range(nP)]
-    want, wd, wl, _ = PO.run_linked(lm, params, end_ns=end_ns, cseed=11)
+    want, wd, wl, _ = LO.run_linked(lm, params, end_ns=end_ns, cseed=11)
     assert np.array_equal(delivered, wd) and np.array_equal(lost, wl) and not over.any()
     for q in range(nP):
         assert_same(outs[q], want[q])

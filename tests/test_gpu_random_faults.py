@@ -1,5 +1,5 @@
 """Node faults on the seeded random models (tests/random_models.py: random_model, random_model_v2, each with the random
-fault plan of random_fault_case) on the device, every replica against the fault oracle (tests/fault_oracle.c), which
+fault plan of random_fault_case) on the device, every replica against the fault oracle (tests/layered_oracle.c), which
 tests/test_faults.py pins against the unmodified reference on the same models.
 
 (a) every model on the auto, warp and thread engines, replica word 0 also against the reference's fixture
@@ -19,7 +19,7 @@ cannot quietly empty itself.  The number of tied replicas is reported as the tes
 import numpy as np
 import pytest
 
-import fault_oracle_lib as FO
+import layered_oracle_lib as LO
 from happysim_b200 import _abi as A, buckets as B, engine, lowering
 from random_models import FAULT_SEEDS_V1, FAULT_SEEDS_V2, random_fault_case, with_faults
 from test_faults import check_random_fault_reference
@@ -83,7 +83,7 @@ def test_every_engine_matches_the_fault_oracle(eng, case, record_property):
     version, seed = case
     fm, end_ns, run_seed = faulted(version, seed)
     kw = dict(seed=run_seed, end_ns=end_ns, n_replicas=5, rid_stride=1, **WHOLE)
-    want = FO.run(fm, engine.make_params(**kw))
+    want = LO.run(fm, engine.make_params(**kw))
     assert int(want["summaries"]["events_processed"].max()) < WHOLE["record_cap"]
     with_ref = version == 2 or seed in FAULT_SEEDS_V1
     eng.upload(fm)
@@ -149,7 +149,7 @@ def test_every_geometry_matches_the_fault_oracle(eng, sm, case, row, record_prop
         check_thread_geometry(li, row, n)
     got = eng.read_outputs()
     assert not (got["summaries"]["status"] & A.HS_ST_QUEUE_OVERFLOW).any(), "queue ring too small for this model"
-    want = FO.run(fm, engine.make_params(**kw))
+    want = LO.run(fm, engine.make_params(**kw))
     assert np.median(want["summaries"]["events_processed"]) > CAPS["record_cap"]       # the rings wrap
     ties = compare_tie_aware(got, want)
     if not ties:

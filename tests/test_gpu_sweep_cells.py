@@ -15,7 +15,7 @@ which tests/test_sweep_cells.py pins to each cell's own single run.
 import numpy as np
 import pytest
 
-import fault_oracle_lib as FO
+import layered_oracle_lib as LO
 import happysim_b200 as hs
 import oracle_lib as O
 from happysim_b200 import _abi as A, buckets as B, distributed as D, engine
@@ -50,7 +50,7 @@ def sm():
 
 
 def oracle(model, p):
-    return FO.run(model, p) if has_kind(model, A.HS_ENT_FAULT) else O.oracle_run_parallel(model, p)
+    return LO.run(model, p) if has_kind(model, A.HS_ENT_FAULT) else O.oracle_run_parallel(model, p)
 
 
 def check(eng, model, got, want):
@@ -235,7 +235,7 @@ def test_faults_in_cells_of_different_concurrency(eng, seed):
     m, end_ns, run_seed, what = cell_case("fault", seed, concurrency="mixed")
     kw = dict(seed=run_seed, end_ns=end_ns, n_replicas=3 * m.n_cells * 4 + 1, replica_index_base=2, replicas_per_cell=3,
               rid_stride=1, flags=FLAGS, queue_ring=RING, **CAPS)
-    want = FO.run(m, O.make_params(**kw))
+    want = LO.run(m, O.make_params(**kw))
     eng.upload(m)
     for e in (1, 3):
         eng.run(engine.make_params(engine=e, **kw))

@@ -108,7 +108,7 @@ def test_read_outputs_gives_the_keys_bucketed_data_reads():
 
 import golden_lib as G  # noqa: E402
 import linked_bucket_models as LB  # noqa: E402
-import linked_fault_oracle_lib as FO  # noqa: E402
+import layered_oracle_lib as LO  # noqa: E402
 import oracle_lib as O  # noqa: E402
 
 
@@ -118,7 +118,7 @@ def _oracle(name, n=1):
     nP = lm.n_partitions
     ps = [O.make_params(seed=kw["seed"], end_ns=kw["end_ns"], n_replicas=n, rid_base=q, rid_stride=nP + 1,
                         **G.linked_caps(z, q)) for q in range(nP)]
-    run = FO.run_linked if any(m.ids_of(A.HS_ENT_FAULT) for m in lm.models) else O.oracle_run_linked
+    run = LO.run_linked if any(m.ids_of(A.HS_ENT_FAULT) for m in lm.models) else O.oracle_run_linked
     outs, delivered, lost, ends = run(lm, ps, end_ns=kw["end_ns"], cseed=kw["seed"])
     assert len(ends) == int(z["total_windows"]) and int(delivered[0]) == int(z["cross_events"])
     return lm, z, outs

@@ -1,5 +1,5 @@
 """Node faults (CrashNode, PauseNode) in the partitions of a linked ParallelSimulation, on the CPU: the fault oracle's
-linked run (tests/linked_fault_oracle.c, hs_fault_oracle_run_linked) against the fixtures recorded from the unmodified
+linked run (tests/layered_oracle.c, hs_layered_oracle_run_linked) against the fixtures recorded from the unmodified
 reference (tests/golden/lfault_*.npz) and the 48 random models (random_linked_faults.npz), the lowering of a
 partition's schedule, the mirror's whole host path on the oracle, and the C-ABI's validation of linked partitions."""
 import os
@@ -7,7 +7,7 @@ import os
 import numpy as np
 import pytest
 
-import linked_fault_oracle_lib as FO
+import layered_oracle_lib as LO
 import golden_lib as G
 import happysim_b200 as hs
 import linked_fault_models as LF
@@ -20,7 +20,7 @@ CASES = G.case_names("lfault_")
 def run_oracle(lm, kw, caps):
     nP = lm.n_partitions
     ps = [O.make_params(seed=kw["seed"], end_ns=kw["end_ns"], rid_base=q, rid_stride=nP + 1, **caps[q]) for q in range(nP)]
-    return FO.run_linked(lm, ps, end_ns=kw["end_ns"], cseed=kw["seed"])
+    return LO.run_linked(lm, ps, end_ns=kw["end_ns"], cseed=kw["seed"])
 
 
 def check_partition(z, q, got, r=0):
@@ -84,7 +84,7 @@ def test_linked_fault_oracle_equals_the_reference_on_random_models(seed):
     lm, end_s, what, _ = LF.random_linked_fault_model(seed)
     nP, end_ns = lm.n_partitions, int(end_s * 1e9)
     ps = [O.make_params(seed=1000 + seed, end_ns=end_ns, rid_base=q, rid_stride=nP + 1) for q in range(nP)]
-    outs, delivered, lost, ends = FO.run_linked(lm, ps, end_ns=end_ns, cseed=1000 + seed)
+    outs, delivered, lost, ends = LO.run_linked(lm, ps, end_ns=end_ns, cseed=1000 + seed)
     top = R["tops"][R["tops"]["seed"] == seed][0]
     rows = R["rows"][R["rows"]["seed"] == seed]
     assert int(delivered[0]) == int(top["delivered"]), what
@@ -223,26 +223,10 @@ def test_partition_validation_accepts_faults_next_to_remote_rows():
         engine.validate_model(m, partition=True)
 
 
-# ---- the mirror's host path, on the fault oracle -------------------------------------------------------------------
-class FaultOracleLinkedRun(O.OracleLinkedRun):
-    """oracle_lib.OracleLinkedRun on the fault oracle: ParallelSimulation's whole host path without a GPU"""
-
-    def run(self, *, seed, end_ns, n_replicas=1, replica_index_base=0, caps=None, flags=A.HS_RUN_ORDER_HASH, queue_ring=0):
-        nP = self.lm.n_partitions
-        caps = caps or {}
-        per = [dict(caps[q] if isinstance(caps, (list, tuple)) else caps) for q in range(nP)]
-        self.calls.append(dict(seed=seed, end_ns=end_ns, n_replicas=n_replicas))
-        ps = [engine.make_params(seed=seed, end_ns=end_ns, n_replicas=n_replicas, rid_base=q, rid_stride=nP + 1,
-                                 replica_index_base=replica_index_base, queue_ring=queue_ring, flags=flags, **per[q])
-              for q in range(nP)]
-        outs, delivered, lost, ends = FO.run_linked(self.lm, ps, end_ns=end_ns, cseed=seed)
-        self.windows = len(ends)
-        return outs, (delivered, lost, np.zeros(n_replicas, np.uint64))
-
-
+# ---- the mirror's host path, on the layered oracle -----------------------------------------------------------------
 def test_run_writes_crashed_and_each_partition_reports_its_cancelled_events(monkeypatch):
     from happysim_b200 import linked
-    monkeypatch.setattr(linked, "LinkedRun", FaultOracleLinkedRun)
+    monkeypatch.setattr(linked, "LinkedRun", LO.OracleCellsLinkedRun)
     fa, fb = hs.FaultSchedule(), hs.FaultSchedule()
     h = fa.add(hs.CrashNode("A.server", at=0.5, restart_at=0.7))
     fb.add(hs.CrashNode("B.sink", at=1.0))

@@ -1,5 +1,5 @@
 """Linked ParallelSimulations as the cells of one ensemble, without a GPU: which configurations share a linked
-topology, the cell oracle (tests/linked_sweep_oracle.c) against the unmodified oracle's standalone run of every cell and
+topology, the cell oracle (tests/layered_oracle.c) against the unmodified oracle's standalone run of every cell and
 against the reference (tests/golden/lsweep_cells.npz), the host path of run_ensemble(cells=) and run_sweep on the
 oracle, and the ABI's refusal of malformed per-cell link tables."""
 import os
@@ -9,6 +9,7 @@ import pytest
 
 import golden_lib as G
 import happysim_b200 as hs
+import layered_oracle_lib as LO
 import linked_fault_models as LF
 import linked_sweep_lib as LS
 import oracle_lib as O
@@ -96,8 +97,7 @@ def _standalone(lm, params, g, *, end_ns, cseed, faults):
         q.n_replicas, q.replica_index_base = 1, g
         ps.append(q)
     if faults:
-        import linked_fault_oracle_lib as FO
-        return FO.run_linked(lm, ps, end_ns=end_ns, cseed=cseed)
+        return LO.run_linked(lm, ps, end_ns=end_ns, cseed=cseed)
     return O.oracle_run_linked(lm, ps, end_ns=end_ns, cseed=cseed)
 
 
@@ -105,7 +105,7 @@ def check_cells_against_standalone(lm, *, seed, end_ns, n, n_cells, rpc, base, f
     celled = LS.celled(lm, seed, n_cells)
     celled.validate()
     ps = LS.partition_params(celled, seed=seed, end_ns=end_ns, n=n, caps=CAPS, replica_index_base=base, replicas_per_cell=rpc)
-    outs, delivered, lost, _ = LS.run_cells(celled, ps, end_ns=end_ns, cseed=seed, replicas_per_cell=rpc)
+    outs, delivered, lost, _ = LO.run_linked(celled, ps, end_ns=end_ns, cseed=seed, replicas_per_cell=rpc)
     cells = LS.cell_of(n, base, rpc, n_cells)
     for r in range(n):
         c = int(cells[r])
@@ -207,7 +207,7 @@ def test_cell_oracle_equals_the_reference_per_configuration(name):
     lm, seed, end_ns, nc = load_sweep_case(z, name)
     caps = sweep_caps(z, name, lm, nc)
     ps = LS.partition_params(lm, seed=seed, end_ns=end_ns, n=nc, caps=caps, rid_stride=0)
-    outs, delivered, lost, ends = LS.run_cells(lm, ps, end_ns=end_ns, cseed=seed, crid_stride=0)
+    outs, delivered, lost, ends = LO.run_linked(lm, ps, end_ns=end_ns, cseed=seed, crid_stride=0)
     assert len(ends) == int(z[f"{name}_c0_windows"])
     check_against_sweep_fixture(z, name, lm, outs, delivered, range(nc))
 
@@ -216,9 +216,9 @@ def test_cell_oracle_equals_the_reference_per_configuration(name):
 
 @pytest.fixture
 def on_oracle(monkeypatch):
-    LS.OracleCellsLinkedRun.runs = []
-    monkeypatch.setattr(linked, "LinkedRun", LS.OracleCellsLinkedRun)
-    return LS.OracleCellsLinkedRun
+    LO.OracleCellsLinkedRun.runs = []
+    monkeypatch.setattr(linked, "LinkedRun", LO.OracleCellsLinkedRun)
+    return LO.OracleCellsLinkedRun
 
 
 def _configs():
@@ -243,7 +243,7 @@ def test_run_ensemble_cells_equal_each_cells_own_ensemble(on_oracle, monkeypatch
         o, d, l_ = own[int(c)]
         LS.assert_replica_equal([outs[k] for k in names], [o[k] for k in names], r, r, f"replica {r}")
         assert (int(delivered[r]), int(lost[r])) == (int(d[r]), int(l_[r]))
-    monkeypatch.setattr(linked, "LinkedRun", LS.OracleCellsLinkedRun)
+    monkeypatch.setattr(linked, "LinkedRun", LO.OracleCellsLinkedRun)
     a = cells[0].run_ensemble(4, 0, cells=cells, replicas_per_cell=rpc)
     b = cells[0].run_ensemble(6, 4, cells=cells, replicas_per_cell=rpc)
     for k in names:

@@ -1,5 +1,5 @@
 """PriorityQueue servers (components/queue_policy.py:189-287) with PriorityByKey priorities, CPU part: the priority
-oracle (tests/priority_oracle.c) against the unmodified reference's fixtures, bit for bit; the lowering's acceptance
+oracle (tests/layered_oracle.c) against the unmodified reference's fixtures, bit for bit; the lowering's acceptance
 and refusals; the C-ABI's validation; sweeps of different priority tables never sharing a launch.  The device engines
 run the same models in tests/test_gpu_priority.py."""
 import math
@@ -11,7 +11,7 @@ import pytest
 import golden_lib as G
 import oracle_lib as O
 import priority_models as PM
-import priority_oracle_lib as PO
+import layered_oracle_lib as LO
 import happysim_b200 as hs
 from happysim_b200 import _abi as A
 from happysim_b200 import api, engine, lowering, results
@@ -37,7 +37,7 @@ def test_fixture_model_is_what_the_generator_built(name):
 def test_oracle_matches_the_reference(name):
     model, kw, z = G.load(f"prio_{name}")
     engine.validate_model(model)
-    G.check_against(z, PO.run(model, fixture_params(z, kw)))
+    G.check_against(z, LO.run(model, fixture_params(z, kw)))
 
 
 def test_fixtures_exercise_what_they_are_named_for():
@@ -70,7 +70,7 @@ def test_windows_resume_with_waiting_requests():
         model, kw, z = G.load(f"prio_{name}")
         end_ns = kw["end_ns"]
         for c in (end_ns // 5 + 7, end_ns // 2 + 3, (4 * end_ns) // 5):
-            part = PO.run(model, O.make_params(seed=kw["seed"], end_ns=end_ns, window_end_ns=c, n_replicas=5))
+            part = LO.run(model, O.make_params(seed=kw["seed"], end_ns=end_ns, window_end_ns=c, n_replicas=5))
             st = part["entity_stats"]
             srv = model.ids_of(A.HS_ENT_SERVER)
             waiting = sum(int(st[r][i]["c0"]) - int(st[r][i]["c2"]) - min(int(model.entities["i0"][i]), int(st[r][i]["c0"]) - int(st[r][i]["c2"]))
@@ -82,7 +82,7 @@ def test_windows_resume_with_waiting_requests():
 def test_oracle_matches_the_reference_on_random_models(seed):
     model, end_s, _ = PM.random_priority_model(seed)
     engine.validate_model(model)
-    out = PO.run(model, O.make_params(seed=int(RANDOM["base_seed"]) + seed, end_ns=int(end_s * 1e9)))
+    out = LO.run(model, O.make_params(seed=int(RANDOM["base_seed"]) + seed, end_ns=int(end_s * 1e9)))
     ws, s = RANDOM[f"s{seed}_summary"][0], out["summaries"][0]
     for f in ("events_processed", "final_time_ns", "order_hash", "heap_left", "n_sink_samples", "n_service_samples"):
         assert int(s[f]) == int(ws[f]), (seed, f)
@@ -224,7 +224,7 @@ def test_same_topology_splits_on_the_priority_table():
 def test_write_back_publishes_the_insert_counter():
     policy = hs.PriorityQueue(capacity=3, key=hs.PriorityByKey([1, 0, 1, 0]))
     model, objs = build(policy)
-    out = PO.run(model, O.make_params(seed=5, end_ns=20 * 10 ** 9, record_cap=4000, sample_cap=4000, service_cap=4000))
+    out = LO.run(model, O.make_params(seed=5, end_ns=20 * 10 ** 9, record_cap=4000, sample_cap=4000, service_cap=4000))
     results.write_back(model, objs, out, 0, hs.Instant)
     i = model.ids_of(A.HS_ENT_SERVER)[0]
     assert policy._insert_counter == objs[i].stats_accepted == int(out["entity_stats"][0][i]["c0"]) > 0

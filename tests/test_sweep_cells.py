@@ -9,7 +9,7 @@ import os
 import numpy as np
 import pytest
 
-import fault_oracle_lib as FO
+import layered_oracle_lib as LO
 import happysim_b200 as hs
 import oracle_lib as O
 from happysim_b200 import _abi as A, api, engine
@@ -28,7 +28,7 @@ def _id(c):
 
 
 def run_oracle(model, p):
-    return FO.run(model, p) if has_kind(model, A.HS_ENT_FAULT) else O.oracle_run(model, p)
+    return LO.run(model, p) if has_kind(model, A.HS_ENT_FAULT) else O.oracle_run(model, p)
 
 
 def launch_shape(seed, n_cells):
